@@ -1,10 +1,11 @@
-"""Headline benchmark: clips/sec of the TimeSformer-B + DistilBERT dual-encoder step on B200.
+"""Headline benchmark: clips/sec of the TimeSformer-B + DistilBERT dual-encoder step on H100.
 
     python bench.py --gpus N --steps K --warmup W [--workload cfg3]      (N > 1: launched by torch.distributed.run)
     python bench.py --impl reference ...                                  (the reference algorithm on the host CPU cores)
+    python bench.py ... --dump-outputs DIR                                (also write the last timed step's results)
 
 Workloads = BASELINE.json `configs` (per-GPU shapes; weak scaling in N):
-  cfg3 (default, the headline)  16f x 224^2, per-GPU batch 64, L=16, EgoNCE over G = 64 N: zero_grad -> FrozenInTime forward
+  cfg3 (default, the headline)  16f x 224^2, per-GPU batch 32, L=16, EgoNCE over G = 32 N: zero_grad -> FrozenInTime forward
                                 -> ONE packed embedding/tag all-gather -> fused similarity + EgoNCE -> backward -> DDP
                                 gradient all-reduce -> AdamW
   cfg2                          the same step at 4 frames (the reference's 4f pretraining shape), per-GPU batch 64
@@ -32,7 +33,8 @@ warnings.simplefilter("ignore")
 WORKLOADS = {
     "cfg2": dict(kind="train", frames=4, batch=64, loss="egonce",
                  metric="clips/sec, 4-frame TimeSformer-B + DistilBERT + EgoNCE training step"),
-    "cfg3": dict(kind="train", frames=16, batch=64, loss="egonce",
+    # batch 32: the step saves ~1.45 GB of activations per 16-frame clip, so 64 clips would not fit an 80 GB H100
+    "cfg3": dict(kind="train", frames=16, batch=32, loss="egonce",
                  metric="clips/sec, 16-frame TimeSformer-B + DistilBERT + EgoNCE training step"),
     "cfg4": dict(kind="train", frames=16, batch=32, loss="maxmargin",
                  metric="clips/sec, 16-frame EPIC-Kitchens MIR fine-tune step (MaxMarginRankingLoss)"),
@@ -57,7 +59,8 @@ def measured_peaks():
     if os.path.exists(path):
         p = json.load(open(path))
         return p, "measured (MEASURED_PEAKS.json)"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback (B200_PROFILING.md)"
+    # H100 SXM data sheet (700 W board): dense bf16 989 TFLOP/s, HBM3 3.35 TB/s -- limits, not reached rates
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "H100 SXM data sheet"
 
 
 def host_cores():
@@ -117,7 +120,7 @@ class ClockSampler:
 
 
 # ----------------------------------------------------------------------------------------------------------------------
-# baselines: the reference's algorithm (oracle port) on the host cores, and in eager PyTorch on the same B200
+# baselines: the reference's algorithm (oracle port) on the host cores, and in eager PyTorch on the same GPU
 # ----------------------------------------------------------------------------------------------------------------------
 def _oracle_step_fn(wl, T, L, batch, device, autocast=False, seed=0):
     """One step of workload `wl` through the oracle port (torch, functional) on `device`; returns (step fn, clips/step)."""
@@ -177,7 +180,7 @@ def cpu_reference_rate(wl, T, L, steps, warmup):
 
 
 def gpu_eager_baseline(wl, T, L, device, budget_s=12.0):
-    """SURVEY.md 8d's "meaningful denominator": the reference's algorithm in eager PyTorch ON THIS B200 (oracle port;
+    """SURVEY.md 8d's "meaningful denominator": the reference's algorithm in eager PyTorch ON THIS GPU (oracle port;
     fp32 = the reference's own precision, then TF32 and bf16 autocast), a few clips, bounded time."""
     out = {"what": "oracle port (reference algorithm, eager PyTorch) on the same GPU", "unit": "clips/s"}
     batch = 8 if wl["kind"] == "train" else 40
@@ -231,10 +234,28 @@ def workload_config(args, wl, world, cpu_sample=False):
                        + (" [CPU arm: bounded sample of 2 clips (training) / 5 clips (inference) per step]" if cpu_sample else ""),
            "global_batch": args.batch * world, "frames": args.frames, "text_len": args.text_len,
            "parallelism": f"dp{world}",
-           "l2_policy": "per-step working set (tens of GB of activations) >> 126 MB L2; no explicit flush needed"}
+           "l2_policy": "per-step working set (tens of GB of activations) >> 50 MB L2; no explicit flush needed"}
     if wl["kind"] == "train":
         cfg["optimizer"] = "AdamW (HF semantics) lr 3e-5"
     return cfg
+
+
+def dump_outputs(path, out, net, train):
+    """What the last timed step computed, as path/<name>.npy.  Training: the loss and, per parameter in named order, 4096
+    entries at fixed seeded positions of the weights AdamW has just updated (5 MB in all); EgoMCQ: scores and argmax."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    if train:
+        np.save(os.path.join(path, "loss.npy"), np.array([out.item()], dtype=np.float64))
+        parts = []
+        for i, (_, p) in enumerate(net.named_parameters()):
+            idx = torch.randint(0, p.numel(), (4096,), generator=torch.Generator().manual_seed(i)).to(p.device)
+            parts.append(p.detach().flatten()[idx].float().cpu())
+        np.save(os.path.join(path, "weights_sample.npy"), torch.cat(parts).numpy())
+    else:
+        scores, pred = out
+        np.save(os.path.join(path, "scores.npy"), scores.float().cpu().numpy())
+        np.save(os.path.join(path, "predictions.npy"), pred.cpu().numpy().astype(np.float64))
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -253,6 +274,9 @@ def main():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-ddp-comm", action="store_true", help="diagnostic: DDP no_sync (no gradient all-reduce)")
     ap.add_argument("--ddp-bf16-compress", action="store_true", help="bf16 gradient-compression DDP comm hook")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last timed step's results to DIR/<name>.npy (training: the loss "
+                         "and a fixed seeded sample of the updated weights; EgoMCQ: scores and predictions)")
     ap.add_argument("--ddp-bucket-mb", type=int, default=0,
                     help="DDP bucket_cap_mb (default: EGOVLP_DDP_BUCKET_MB or 2048 = ONE gradient bucket all-reduced after "
                          "the backward; 25 = torch's default overlapped buckets)")
@@ -279,6 +303,7 @@ def main():
     if world > 1:
         dist.init_process_group("nccl", device_id=dev)
     assert args.warmup >= 3 or args.steps <= 2, "use at least 3 warm-up steps for a reportable number"
+    torch.manual_seed(0)                                     # text-tower dropout seeds: identical runs for identical args
 
     B, T, L = args.batch, args.frames, args.text_len
     train = wl["kind"] == "train"
@@ -343,13 +368,12 @@ def main():
     def egomcq_step(data):
         with torch.no_grad():
             t, v = net(data)                                 # [Q, 256], [5 Q, 256]
-            scores, pred = egomcq_predict(t, v.view(t.shape[0], 5, -1))
-        return pred
+            return egomcq_predict(t, v.view(t.shape[0], 5, -1))      # scores [Q, 5], predictions [Q]
 
     step = train_step if train else egomcq_step
 
     def result_to_host(out):
-        return out.item() if train else out.cpu()            # loss value / the [Q] predictions
+        return out.item() if train else out[1].cpu()         # loss value / the [Q] predictions
 
     def barrier():
         if world > 1:
@@ -382,6 +406,8 @@ def main():
     launches = _lib.launch_count()
     clocks = sampler.stop() if rank == 0 else None
     result = result_to_host(out)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, out, net, train)
     ms_per_step = ms_total / args.steps
     value = B * world * args.steps / (ms_total / 1e3)
 
@@ -450,14 +476,6 @@ def main():
         peak_hbm = peaks["hbm_gbs"]
         g_flops, g_ms, g_calls = prof.get("gemm", (0.0, 0.0, 0))
         achieved = g_flops / (g_ms / 1e3) / 1e12 if g_ms > 0 else None
-        # DRAM bytes of the same launches from the committed ncu capture (valid for the default workload only)
-        traffic, traffic_src = None, None
-        tpath = os.path.join(ROOT, "profiles", "r1_gemm_dram_traffic.json")
-        if os.path.exists(tpath) and (args.workload, args.batch, T, L) == ("cfg3", 64, 16, 16):
-            with open(tpath) as f:
-                tj = json.load(f)
-            traffic = tj["dram_bytes_per_step"] / tj["launches_per_step"]
-            traffic_src = "profiles/r1_gemm_dram_traffic.json (ncu dram__bytes_read+write.sum, mean per GEMM launch of one step)"
         hbm = {}
         for kind, (nbytes, ms, calls) in sorted(prof.items()):
             if kind == "gemm" or ms <= 0:
@@ -475,10 +493,9 @@ def main():
                 ("loss" if train else "pred_checksum"): (result if train else int(result.sum())),
                 "step_flop_fraction_of_peak": value / world * f_clip / (peak_tf * 1e12),
                 "gflop_per_clip_step": f_clip / 1e9,
-                "roofline": {"bound": "tensor", "kernel": "gemm_bf16_tcgen05_kernel (all fwd/dgrad/wgrad launches)",
+                "roofline": {"bound": "tensor", "kernel": "gemm_bf16_wgmma_kernel (all fwd/dgrad/wgrad launches)",
                              "achieved": achieved, "peak": peak_tf, "unit": "TFLOP/s",
-                             "frac": achieved / peak_tf if achieved else None, "traffic": traffic,
-                             "traffic_unit": "bytes per launch", "traffic_source": traffic_src,
+                             "frac": achieved / peak_tf if achieved else None,
                              "algorithmic_flop_per_launch": g_flops / g_calls if g_calls else None,
                              "launches_per_step": g_calls / args.steps, "share_of_step": g_ms / ms_total,
                              "peak_source": peak_src + ", sustained bf16 (kernel timed inside a long step)"},

@@ -1,4 +1,4 @@
-"""egovlp_b200: B200-native implementation of the EgoVLP dual-encoder pretraining hot path.
+"""egovlp_b200: H100-native (sm_90a) implementation of the EgoVLP dual-encoder pretraining hot path.
 
     from egovlp_b200.model.model import FrozenInTime, sim_matrix
     from egovlp_b200.model.loss import EgoNCE, NormSoftmaxLoss, MaxMarginRankingLoss
@@ -16,8 +16,9 @@ __version__ = "0.1.0"
 def _one_bucket_ddp():
     """Make `DistributedDataParallel(...)` calls that do not choose a bucket size (the reference's
     base/base_trainer.py:254-258) use ONE gradient bucket all-reduced after the backward: with this package's persistent
-    one-CTA-per-SM GEMMs, torch's default overlapped 25 MB buckets cost more than they hide (8 x B200: 2402 vs 2442
-    clips/s, profiles/r2_scaling_8gpu.json).  EGOVLP_DDP_BUCKET_MB overrides (25 = torch's default)."""
+    one-CTA-per-SM GEMMs, NCCL's CTAs competing with the persistent GEMMs of the backward cost more than overlapped
+    25 MB buckets hide (measured on an earlier multi-GPU Blackwell build; not re-measured on H100).
+    EGOVLP_DDP_BUCKET_MB overrides (25 = torch's default)."""
     import functools
     import os
     import torch

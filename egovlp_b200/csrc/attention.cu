@@ -11,9 +11,9 @@
 // query r may attend key c iff  gid[c] == gid[r]  or c is the CLS key; the CLS query attends every patch key
 // of the CTA plus the CLS key in the first group only, and its per-group (max, sum, acc) partials are merged by
 // a tiny second kernel -- so the CLS-over-all-S row (:112) costs no extra pass over K/V.
-// Math: bf16 mma.sync m16n8k16 with fp32 accumulation + fp32 online softmax (exp2).  This op is HBM-bound on
-// B200 (<= 98 FLOP/B, SURVEY.md section 8d), so the legacy tensor path is sufficient to sit on the HBM roofline;
-// the tcgen05 pipeline is reserved for the GEMMs that carry 96% of the FLOPs.
+// Math: bf16 mma.sync m16n8k16 with fp32 accumulation + fp32 online softmax (exp2).  At head_dim 64 this op does
+// <= 98 FLOP per byte it moves (SURVEY.md section 8d): register-resident mma.sync tiles keep S and P out of shared
+// memory, and the wgmma pipeline is kept for the GEMMs that carry 96% of the FLOPs.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -21,14 +21,10 @@
 
 namespace egovlp {
 
-// tcgen05 / TMEM space-attention forward (attention_tc.cu)
-bool space_attn_tc_supported(int N);
-// tcgen05 / TMEM space-attention backward (attention_tc_bwd.cu)
-bool space_attn_bwd_tc_supported(int N);
-int space_attn_bwd_tc(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv, float* dcls,
-                      int B, int T, int N, int H, float q_scale, cudaStream_t st);
-int space_attn_fwd_tc(const void* qkv, void* out, float* lse, float* cls_part, int B, int T, int N, int H,
-                      cudaStream_t st);
+// wgmma space-attention forward (attention_wgmma.cu), opt-in
+bool space_attn_wgmma_supported(int N);
+int space_attn_fwd_wgmma(const void* qkv, void* out, float* lse, float* cls_part, int B, int T, int N, int H,
+                         cudaStream_t st);
 
 namespace {
 
@@ -1244,8 +1240,8 @@ extern "C" int egovlp_divided_attn_fwd(const void* qkv, void* out, float* lse, f
     KERN<<<grid, W * 32, smem, st>>>(tm, q, o, lse, cls_part, G, ##__VA_ARGS__);                              \
   } while (0)
   const bool generic = force_generic() || (mode == 0 && !time_fast_ok(G));
-  if (!generic && mode == 1 && space_attn_tc_supported(N)) {     // tcgen05 / TMEM kernel
-    rc = space_attn_fwd_tc(qkv, out, lse, cls_part, B, T, N, H, st);
+  if (!generic && mode == 1 && space_attn_wgmma_supported(N)) {
+    rc = space_attn_fwd_wgmma(qkv, out, lse, cls_part, B, T, N, H, st);
     if (rc) return rc;
   } else if (generic) {
     if (G.NPAD > 128) LAUNCH_FWD((divided_attn_fwd_kernel<7, 2>), 7);
@@ -1291,10 +1287,7 @@ extern "C" int egovlp_divided_attn_bwd(const void* qkv, const void* out, const v
     KERN<<<grid, W * 32, smem, st>>>(tmq, tmd, q, o, d_o, lse, dq, dcls_ws, q_scale, G, ##__VA_ARGS__);       \
   } while (0)
   const bool generic = force_generic() || (mode == 0 && !time_fast_ok(G));
-  if (!generic && mode == 1 && space_attn_bwd_tc_supported(N)) {     // tcgen05 / TMEM kernel (default at N = 196)
-    rc = space_attn_bwd_tc(qkv, out, dout, lse, dqkv, dcls_ws, B, T, N, H, q_scale, st);
-    if (rc) return rc;
-  } else if (generic) {
+  if (generic) {
     if (G.NPAD > 128) LAUNCH_BWD((divided_attn_bwd_kernel<7, 2>), 7);
     else LAUNCH_BWD((divided_attn_bwd_kernel<4, 3>), 4);
   } else if (mode == 1) {     // space: 2 CTAs / SM (4 x 26 KB tiles each, no staging)

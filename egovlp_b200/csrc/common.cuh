@@ -1,4 +1,4 @@
-// Shared device helpers for the sm_100a kernels: mbarrier / TMA / tcgen05 / TMEM PTX wrappers,
+// Shared device helpers for the sm_90a kernels: mbarrier / TMA / wgmma PTX wrappers,
 // warp reductions, bf16 packing.  Hand-written inline PTX (no CUTLASS templates).
 #pragma once
 #include <cuda.h>
@@ -76,31 +76,18 @@ __device__ __forceinline__ float gelu_erf_grad(float x) {
 }
 
 // ------------------------------------------------------------------------------------------
-// packed fp32x2 arithmetic (sm_100: FFMA2 / FMUL2 / FADD2 -- two fp32 lanes per instruction; issue-bound
-// epilogues and softmax loops use it to halve their FMA-pipe instruction count)
+// fp32 pairs.  Epilogues and softmax loops are written two elements at a time; sm_90 has no packed fp32x2
+// instructions, so each helper is two scalar round-to-nearest operations (the _rn intrinsics keep the compiler from
+// contracting a multiply and an add into an FMA, so results do not depend on how a caller's pairs are combined).
 // ------------------------------------------------------------------------------------------
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 pk2(float a, float b) {
-  f32x2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b));
-  return r;
-}
-__device__ __forceinline__ void up2(f32x2 v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
+typedef float2 f32x2;
+__device__ __forceinline__ f32x2 pk2(float a, float b) { return make_float2(a, b); }
+__device__ __forceinline__ void up2(f32x2 v, float& a, float& b) { a = v.x; b = v.y; }
 __device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
-  f32x2 d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
-__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) {
-  f32x2 d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) {
-  f32x2 d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
+__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 
 // ------------------------------------------------------------------------------------------
 // Counter-based RNG for dropout: Philox4x32-10 keyed by (seed, site), counter = element group.  Stateless, so the
@@ -165,6 +152,19 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   }
 }
 
+// Same bound without the printf call site: a call inside a wgmma pipeline makes ptxas serialise every wgmma of the
+// kernel, and makes the caller's live registers spill around it.  The clock is only read every 1024 polls.
+__device__ __forceinline__ void mbar_wait_nocall(uint32_t bar, uint32_t parity) {
+  if (mbar_try_wait(bar, parity)) return;
+  const long long t0 = clock64();
+  for (;;) {
+#pragma unroll 1
+    for (int i = 0; i < 1024; ++i)
+      if (mbar_try_wait(bar, parity)) return;
+    if (clock64() - t0 > 4000000000LL) __trap();
+  }
+}
+
 // ------------------------------------------------------------------------------------------
 // TMA (cp.async.bulk.tensor)
 // ------------------------------------------------------------------------------------------
@@ -197,50 +197,23 @@ __device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* m, 
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
       : "memory");
 }
+// Multicast load: the box lands at the same smem offset in every CTA of `mask` (cluster ranks) and completes
+// transaction bytes on the mbarrier at the same offset in each of them.
+__device__ __forceinline__ void tma_load_2d_multicast(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1,
+                                                      uint16_t mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "h"(mask)
+      : "memory");
+}
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
 // ------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// thread-block clusters
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]; issued by ONE thread.
-__device__ __forceinline__ void umma_bf16_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// A operand from TMEM (bf16 packed, written with tcgen05.st), B from smem.
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05 ops of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-// ---- CTA-pair (cta_group::2) variants: one MMA spans two SMs of a cluster; issued by the even ("leader") CTA ----
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -249,109 +222,41 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
+// address of the same shared-memory offset in the CTA of the given cluster rank
 __device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t cta_rank) {
   uint32_t r;
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(cta_rank));
   return r;
 }
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
   asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
 }
-// TMA load issued by either CTA of the pair; the transaction bytes are credited to the LEADER CTA's mbarrier
-// (same smem offset, peer bit 24 cleared -- the convention CUTLASS's SM100_TMA_2SM_LOAD uses).
-__device__ __forceinline__ void tma_load_2d_2sm(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar & 0xFEFFFFFFu), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_bf16_ss_2cta(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                                  uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive (once all earlier tcgen05 ops of this thread are done) on the mbarrier at this smem offset in BOTH CTAs
-__device__ __forceinline__ void umma_commit_2cta(uint32_t bar) {
-  const uint16_t mask = 3;
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(bar), "h"(mask)
-      : "memory");
+
+// ------------------------------------------------------------------------------------------
+// wgmma (sm_90a warpgroup MMA): issued by all 128 threads of a warpgroup, accumulators in registers
+// ------------------------------------------------------------------------------------------
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Pins accumulator registers in place around wgmma issue / wait, so that the compiler neither reads them before the
+// asynchronous MMA has written them nor moves other uses across the wait.
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// Instruction descriptor, kind::f16, bf16 x bf16 -> f32 (cute/arch/mma_sm100_desc.hpp InstrDescriptor bit layout).
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, bool a_mn_major, bool b_mn_major) {
-  return (1u << 4)                          // c_format  = F32
-         | (1u << 7)                        // a_format  = BF16
-         | (1u << 10)                       // b_format  = BF16
-         | ((a_mn_major ? 1u : 0u) << 15)   // a_major
-         | ((b_mn_major ? 1u : 0u) << 16)   // b_major
-         | (uint32_t(N >> 3) << 17)         // n_dim
-         | (uint32_t(M >> 4) << 24);        // m_dim
-}
-
-// Shared-memory matrix descriptor, SWIZZLE_128B, version 1 (Blackwell).  Offsets in bytes.
+// Shared-memory matrix descriptor (sm_90 wgmma), SWIZZLE_128B.  Offsets in bytes.
+// K-major tiles: 128-byte rows, 8-row core groups SBO = 1024 apart (LBO unused).  MN-major tiles: [k][64 mn] slabs of
+// 128-byte rows, 8-k-row groups SBO = 1024 apart, slabs of 64 mn LBO apart.
 __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= uint64_t((saddr >> 4) & 0x3FFF);
   d |= uint64_t((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= uint64_t((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= uint64_t(1) << 46;  // version = 1
-  d |= uint64_t(2) << 61;  // layout_type = SWIZZLE_128B
+  d |= uint64_t(1) << 62;  // layout_type = SWIZZLE_128B
   return d;
-}
-
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive 32-bit columns (thread i <- lane base+i).
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,"
-      "%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x8(uint32_t taddr, uint32_t (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// registers -> TMEM, 32 lanes x 16 columns
-__device__ __forceinline__ void tmem_st_32x32b_x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-        "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
 }
 
 // ------------------------------------------------------------------------------------------

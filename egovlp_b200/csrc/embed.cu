@@ -1,4 +1,4 @@
-// Patch-embedding front end of the video tower: im2col (+fp32->bf16) feeding the tcgen05 GEMM, the
+// Patch-embedding front end of the video tower: im2col (+fp32->bf16) feeding the wgmma GEMM, the
 // CLS / positional / temporal embedding table its epilogue adds, and the backward reductions.
 // Replaces VideoPatchEmbed.forward + the embedding assembly (model/video_transformer.py:72-77, 304-321):
 // Conv2d(k16,s16) == GEMM over unfolded patches; cls cat + tiled pos_embed + repeat_interleaved temporal_embed

@@ -40,7 +40,10 @@ layernorm_fwd_kernel(const float* __restrict__ x, long long ldx, const float* __
       v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
     }
   }
-  const float mean = warp_sum(s) / D;
+  // 1/D correctly rounded and explicit roundings: the same arithmetic as the pipelined kernel (whose D is a constant),
+  // so a row's result does not depend on which kernel the row count selects
+  const float inv_d = __frcp_rn((float)D);
+  const float mean = __fmul_rn(warp_sum(s), inv_d);
   float q = 0.f;
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
@@ -50,7 +53,7 @@ layernorm_fwd_kernel(const float* __restrict__ x, long long ldx, const float* __
       q += a * a + b * b + cc * cc + d * d;
     }
   }
-  const float rstd = rsqrtf(warp_sum(q) / D + eps);
+  const float rstd = rsqrtf(__fmaf_rn(warp_sum(q), inv_d, eps));
   if (lane == 0) {
     if (mean_out) mean_out[row] = mean;
     if (rstd_out) rstd_out[row] = rstd;
@@ -131,7 +134,8 @@ layernorm_bwd_kernel(const void* __restrict__ dy_, int dy16, long long lddy, con
         s2 += dyv[i].x * xh[i].x + dyv[i].y * xh[i].y + dyv[i].z * xh[i].z + dyv[i].w * xh[i].w;
       }
     }
-    const float c1 = warp_sum(s1) / D, c2 = warp_sum(s2) / D;
+    const float inv_d = __frcp_rn((float)D);      // as in the pipelined kernel
+    const float c1 = __fmul_rn(warp_sum(s1), inv_d), c2 = __fmul_rn(warp_sum(s2), inv_d);
 #pragma unroll
     for (int i = 0; i < NV; ++i) {
       const int c = (i * 32 + lane) * 4;
@@ -263,7 +267,7 @@ layernorm_bwd_pipe_kernel(const uint8_t* __restrict__ dy, int dy16, const float*
         s1 += dyv[i].x + dyv[i].y + dyv[i].z + dyv[i].w;
         s2 += dyv[i].x * xh[i].x + dyv[i].y * xh[i].y + dyv[i].z * xh[i].z + dyv[i].w * xh[i].w;
       }
-      const float c1 = warp_sum(s1) * (1.f / D), c2 = warp_sum(s2) * (1.f / D);
+      const float c1 = __fmul_rn(warp_sum(s1), 1.f / D), c2 = __fmul_rn(warp_sum(s2), 1.f / D);
 #pragma unroll
       for (int i = 0; i < NV; ++i) {
         const int c = (i * 32 + lane) * 4;
@@ -352,14 +356,14 @@ layernorm_fwd_pipe_kernel(const float* __restrict__ x, const float* __restrict__
         v[i] = *reinterpret_cast<const float4*>(s_x + (i * 32 + lane) * 16);
         s += v[i].x + v[i].y + v[i].z + v[i].w;
       }
-      const float mu = warp_sum(s) * (1.f / D);
+      const float mu = __fmul_rn(warp_sum(s), 1.f / D);
       float q = 0.f;
 #pragma unroll
       for (int i = 0; i < NV; ++i) {
         const float a = v[i].x - mu, b = v[i].y - mu, c = v[i].z - mu, d = v[i].w - mu;
         q += a * a + b * b + c * c + d * d;
       }
-      const float rs = rsqrtf(warp_sum(q) * (1.f / D) + eps);
+      const float rs = rsqrtf(__fmaf_rn(warp_sum(q), 1.f / D, eps));
       if (lane == 0) {
         if (mean_out) mean_out[row] = mu;
         if (rstd_out) rstd_out[row] = rs;

@@ -1,7 +1,7 @@
 // Text-tower specific kernels (DistilBERT, transformers modeling_distilbert.py; call sites model/model.py:117-138):
 // embedding gather (+positions), key-padding-masked self-attention for short sequences (L <= 128), and the
 // CLS -> ReLU gather in front of txt_proj (model/model.py:73-75,125).  The Linear / LayerNorm / GELU work of the
-// tower runs on the shared tcgen05 GEMM and LayerNorm kernels.  <0.4% of the step's FLOPs: fp32 CUDA-core math.
+// tower runs on the shared wgmma GEMM and LayerNorm kernels.  <0.4% of the step's FLOPs: fp32 CUDA-core math.
 #include "common.cuh"
 #include "egovlp_b200.h"
 

@@ -1,5 +1,5 @@
 """Data-parallel plumbing of the step: the embedding / tag all-gather with the reference's local-slice backward,
-packed into ONE collective, and the B200-first fused training step.
+packed into ONE collective, and the fused training step.
 
 Reference semantics (trainer/trainer_egoclip.py:11-27, 125-135): every rank gathers video/text embeddings and
 verb/noun tag vectors, computes the full [G, G] loss redundantly, and back-propagates only its own B rows (no
@@ -68,7 +68,7 @@ class PackedGather(torch.autograd.Function):
 
 
 def egoclip_step_loss(model, loss_fn, data):
-    """Forward of one EgoClip pretraining step, B200-first: model -> ONE packed gather -> ONE fused similarity + EgoNCE
+    """Forward of one EgoClip pretraining step, fused: model -> ONE packed gather -> ONE fused similarity + EgoNCE
     kernel reading the gathered buffer in place (positives from bit-packed tags), whose backward kernel emits the local
     gradient slice.  Equivalent to trainer/trainer_egoclip.py:125-135."""
     text_embeds, video_embeds = model(data)

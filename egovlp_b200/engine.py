@@ -4,7 +4,7 @@ torch supplies device buffers, the current stream and the autograd graph (so DDP
 reference trainer keep working); every FLOP below runs in libegovlp_b200.so through `ops`.
 
 Numerics layout: residual stream and LayerNorm statistics in fp32, GEMM operands in bf16 (fp32 accumulation in
-TMEM), attention probabilities never leave the SM, losses in fp32.  fp32 master parameters are the autograd
+wgmma registers), attention probabilities never leave the SM, losses in fp32.  fp32 master parameters are the autograd
 leaves; their bf16 GEMM copies come from `Bf16Cache` (refreshed when a parameter's version changes).
 """
 import functools
@@ -228,11 +228,12 @@ def _sm_count(device_index):
 
 
 @functools.lru_cache(maxsize=None)
-def _split_for(n_out, n_in, k_rows, n_sm=148):
+def _split_for(n_out, n_in, k_rows, n_sm=132):
     """Split-K factor of a weight-gradient GEMM (one persistent CTA per SM, 128 x 256 tiles, 64-row k-blocks): the split
     whose (tiles x splits) units fill whole waves of the grid.  Cost model = waves x (k-blocks per unit + 4 for the
     pipeline fill and the atomic epilogue that the next unit cannot hide); the smallest split within 3 % of the best
-    (fewer fp32 atomics).  round(400 / tiles) left the 54-tile qkv gradient at 2.55 waves (378 units on 148 SMs)."""
+    (fewer fp32 atomics).  round(400 / tiles) leaves the 72-tile fc1 gradient at 6 splits = 3.27 waves on 132 SMs
+    (0.82 of the occupied waves filled); this rule picks 9 (4.91 waves, 0.98 filled)."""
     tiles = ((n_out + 127) // 128) * ((n_in + 255) // 256)
     num_kb = (k_rows + 63) // 64
     if os.environ.get("EGOVLP_WGRAD_SPLIT", "waves") == "legacy":       # A/B knob: the round-1 rule

@@ -1,7 +1,7 @@
 """Dense feature extraction with the dual encoder (SURVEY.md 8f row 4): the loops of the reference's
 run/test_nlq.py:60-109 (also run/test_mq.py) as library functions.  The reference pushes windows through
 `model.compute_video` four at a time (`batch = 4`, :78); per-window results do not depend on the batch (every kernel
-on the forward path is row-independent and the forward GEMMs use no split-K), so a B200-sized batch gives
+on the forward path is row-independent and the forward GEMMs use no split-K), so a large batch gives
 bit-identical features."""
 import torch
 

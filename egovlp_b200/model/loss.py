@@ -36,7 +36,7 @@ class EgoNCE(nn.Module):
         return engine.NceLossFn.apply(x, mask, self.temperature)
 
     def fused(self, text_embeds, video_embeds, verb_vec, noun_vec):
-        """B200-first entry: gathered embeddings + multi-hot tags -> loss, without materialising the
+        """Fused entry: gathered embeddings + multi-hot tags -> loss, without materialising the
         verb/noun similarity matrices (positives from bit-packed tag co-occurrence)."""
         G, Cc = text_embeds.shape
         if ops.egonce_fused_supported(G, Cc) and video_embeds.shape[1] == Cc:      # ONE kernel per direction

@@ -1,4 +1,4 @@
-"""FrozenInTime dual encoder + sim_matrix on the B200 kernels.
+"""FrozenInTime dual encoder + sim_matrix on the project's H100 kernels.
 
 API mirror of the reference's model/model.py: FrozenInTime(video_params, text_params, projection_dim,
 load_checkpoint, projection, load_temporal_fix), forward(data, video_only, return_embeds), compute_text,

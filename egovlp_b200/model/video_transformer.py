@@ -1,4 +1,4 @@
-"""Space-time video transformer ("frozen-in-time" TimeSformer-B variant) on the B200 kernels.
+"""Space-time video transformer ("frozen-in-time" TimeSformer-B variant) on the project's H100 kernels.
 
 API mirror of the reference's model/video_transformer.py (SpaceTimeTransformer, SpaceTimeBlock, VarAttention,
 Mlp, VideoPatchEmbed): same constructor arguments, attribute names and state_dict keys, so checkpoints and the

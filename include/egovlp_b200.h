@@ -1,4 +1,4 @@
-/* egovlp_b200 — C-ABI of the B200-native EgoVLP hot path (libegovlp_b200.so).
+/* egovlp_b200 — C-ABI of the H100-native (sm_90a) EgoVLP hot path (libegovlp_b200.so).
  *
  * The reference (showlab/EgoVLP) has no FFI layer: its hot path is Python over torch ops
  * (SURVEY.md section 8b).  This header is the boundary a maintainer binds instead of those torch
@@ -32,7 +32,7 @@ const char* egovlp_last_error(void);
 int egovlp_abi_version(void);
 
 /* ------------------------------------------------------------------------------------------------
- * GEMM  D[m,n] = epi( sum_k A[m,k] * B[n,k] ),  bf16 operands, fp32 accumulation (tcgen05/TMEM).
+ * GEMM  D[m,n] = epi( sum_k A[m,k] * B[n,k] ),  bf16 operands, fp32 accumulation (wgmma).
  * Replaces nn.Linear forward/backward everywhere on the path: model/video_transformer.py:41-52
  * (Mlp), :88-89,103,135 (qkv/proj), :70,76 (patch-embed conv as GEMM); DistilBERT q/k/v/out_lin,
  * ffn.lin1/lin2; model/model.py:72-79 (projections); and autograd's dgrad/wgrad of each.

@@ -192,7 +192,7 @@ def test_wgrad_split_k_fills_whole_waves(monkeypatch):
     from egovlp_b200 import engine
     monkeypatch.delenv("EGOVLP_WGRAD_SPLIT", raising=False)
     engine._split_for.cache_clear()
-    n_sm = 148
+    n_sm = 132                                              # H100 SXM
     for n_out, n_in in ((2304, 768), (768, 768), (3072, 768), (768, 3072), (256, 768), (768, 256)):
         for rows in (64 * 3137, 64 * 785, 32 * 3137, 8 * 3137):
             s = engine._split_for(n_out, n_in, rows, n_sm)
@@ -205,9 +205,9 @@ def test_wgrad_split_k_fills_whole_waves(monkeypatch):
             assert units / (-(-units // n_sm) * n_sm) >= 0.9, (n_out, n_in, rows, s)
     # 1024 text tokens: 16 k-blocks only -- still more than one unit per tile
     assert engine._split_for(768, 768, 1024, n_sm) > 1
-    # the measured case: qkv gradient at 64 clips x 16 frames -> 8 splits (432 units = 2.92 waves), not 7 (2.55 waves)
-    assert engine._split_for(2304, 768, 64 * 3137, n_sm) == 8
+    # fc1 weight gradient at 64 clips x 16 frames: 9 splits (648 units = 4.91 waves), not 6 (432 units = 3.27 waves)
+    assert engine._split_for(3072, 768, 64 * 3137, n_sm) == 9
     monkeypatch.setenv("EGOVLP_WGRAD_SPLIT", "legacy")
     engine._split_for.cache_clear()
-    assert engine._split_for(2304, 768, 64 * 3137, n_sm) == 7
+    assert engine._split_for(3072, 768, 64 * 3137, n_sm) == 6
     engine._split_for.cache_clear()

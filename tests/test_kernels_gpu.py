@@ -14,8 +14,9 @@ def ops():
 
 @pytest.fixture(params=["pair", "single"])
 def gemm_mode(request, monkeypatch):
-    """Run every GEMM test on both tile schedulers: CTA-pair 256x256 (default for N % 256 == 0) and single-CTA."""
-    monkeypatch.setenv("EGOVLP_GEMM_1CTA", "1" if request.param == "single" else "0")
+    """Run every GEMM test on both tile schedulers: single CTAs (the default) and CTA pairs (a 2-CTA cluster, 256 x 256
+    tile, B multicast; taken by K-major A with N % 256 == 0 under EGOVLP_GEMM_PAIR=1)."""
+    monkeypatch.setenv("EGOVLP_GEMM_PAIR", "1" if request.param == "pair" else "0")
     return request.param
 
 
@@ -120,7 +121,7 @@ def test_gemm_epilogues(ops, gemm_mode):
 
 @pytest.mark.parametrize("M,N,K", [(1570, 768, 256), (515, 3072, 768), (4099, 1024, 128)])
 def test_gemm_specialised_epilogues_match_the_generic_one(ops, monkeypatch, M, N, K):
-    """The CTA-pair kernels carry compile-time specialised epilogues for the step's hot forms (bias -> bf16, GELU + GELU',
+    """The K-major-A kernels carry compile-time specialised epilogues for the step's hot forms (bias -> bf16, GELU + GELU',
     x aux, bias + fp32 residual -> fp32); EGOVLP_GEMM_GENERIC_EPI=1 routes the same calls through the generic epilogue.
     Same arithmetic in the same order: the results must be bit-identical (ragged last m-block, several tiles per CTA)."""
     a, b = mk((M, K), 30), mk((N, K), 31, 0.06)
@@ -238,14 +239,12 @@ def test_divided_attention_fwd_bwd(ops, B, T, N, H, mode, generic, monkeypatch):
     """Both implementations (specialised span kernels; generic group-id kernels) against the oracle's restatement
     of VarAttention's core, incl. partially filled time groups (N not a multiple of the patches per group)."""
     from oracle import reference_port as rp
-    # False: default dispatch (mma.sync span kernels, tcgen05 space backward); "tc": + tcgen05/TMEM space forward;
-    # True: generic group-id kernels; "w8": 8-warp time backward and the mma.sync space backward (EGOVLP_ATTN_TC_BWD=0).
-    # (3, 16, 196, 8, 1) has 384 groups: the persistent tcgen05 kernels loop 2-3 times per CTA (ring / parity logic);
-    # (2, 4, 150, 2, 1) exercises a short second tile (151 keys -> 160 padded, W1 = 32).
+    # False: default dispatch (mma.sync span kernels); True: generic group-id kernels; "tc": + the wgmma space-attention
+    # forward (128 < N + 1 <= 208); "w8": the 8-warp time backward.
+    # (3, 16, 196, 8, 1) has 384 groups; (2, 4, 150, 2, 1) has 151 keys: a partly filled last key tile.
     monkeypatch.setenv("EGOVLP_ATTN_GENERIC", "1" if generic is True else "0")
     monkeypatch.setenv("EGOVLP_ATTN_TC", "1" if generic == "tc" else "0")
     monkeypatch.setenv("EGOVLP_ATTN_TIME_BWD_WARPS", "8" if generic == "w8" else "4")   # both time-backward shapes
-    monkeypatch.setenv("EGOVLP_ATTN_TC_BWD", "0" if generic == "w8" else "1")
     S, D = 1 + T * N, 64 * H
     qkv = mk((B * S, 3 * D), 50 + T + mode, 1.0)
     scale = 0.125

@@ -1,4 +1,4 @@
-"""Micro-benchmark of the tcgen05 GEMM on the shapes of the 16-frame step (B=64 -> M=200768 tokens)."""
+"""Micro-benchmark of the wgmma GEMM on the shapes of the 16-frame step (B=64 -> M=200768 tokens)."""
 import json
 import sys
 import os

@@ -1,5 +1,5 @@
 """Same-box GPU baseline (SURVEY.md 8d): the oracle port -- the reference's algorithm restated op for op in eager
-PyTorch (oracle/reference_port.py) -- timed ON the B200 in fp32 (TF32 off / on) and under bf16 autocast, fwd + bwd +
+PyTorch (oracle/reference_port.py) -- timed on the GPU in fp32 (TF32 off / on) and under bf16 autocast, fwd + bwd +
 torch AdamW, at the largest per-GPU batch the eager path's fp32 activations allow.  This is a measurement tool, not a
 product path: it is the "what the reference's own code path costs on this GPU" denominator quoted in DESIGN.md.
 

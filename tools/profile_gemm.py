@@ -1,4 +1,4 @@
-"""Tiny driver for ncu: a few launches of the tcgen05 GEMM on the step's dominant shapes."""
+"""Tiny driver for ncu: a few launches of the wgmma GEMM on the step's dominant shapes."""
 import os
 import sys
 import torch
