@@ -44,8 +44,8 @@ static EncodeTiledFn encode_fn() {
   return fn;
 }
 
-int make_tmap_nd_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides,
-                      const uint32_t* box, bool swizzle128) {
+static int make_tmap_nd(CUtensorMap* out, CUtensorMapDataType dtype, uint64_t esize, const void* base, int rank,
+                        const uint64_t* dims, const uint64_t* strides, const uint32_t* box, bool swizzle128) {
   EncodeTiledFn fn = encode_fn();
   if (!fn) {
     set_last_error("cuTensorMapEncodeTiled entry point unavailable");
@@ -57,9 +57,9 @@ int make_tmap_nd_bf16(CUtensorMap* out, const void* base, int rank, const uint64
     gdim[i] = dims[i];
     bx[i] = box[i];
     estr[i] = 1;
-    if (i > 0) gstr[i - 1] = strides[i] * 2;
+    if (i > 0) gstr[i - 1] = strides[i] * esize;
   }
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(base), gdim, gstr, bx, estr,
+  CUresult r = fn(out, dtype, rank, const_cast<void*>(base), gdim, gstr, bx, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
@@ -71,12 +71,25 @@ int make_tmap_nd_bf16(CUtensorMap* out, const void* base, int rank, const uint64
   return EGOVLP_OK;
 }
 
+int make_tmap_nd_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides,
+                      const uint32_t* box, bool swizzle128) {
+  return make_tmap_nd(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, base, rank, dims, strides, box, swizzle128);
+}
+
 int make_tmap_2d_bf16(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows,
                       uint32_t box_cols) {
   const uint64_t dims[2] = {cols, rows};
   const uint64_t strides[2] = {1, ld};
   const uint32_t box[2] = {box_cols, box_rows};
   return make_tmap_nd_bf16(out, base, 2, dims, strides, box, true);
+}
+
+int make_tmap_2d_f32(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows,
+                     uint32_t box_cols) {
+  const uint64_t dims[2] = {cols, rows};
+  const uint64_t strides[2] = {1, ld};
+  const uint32_t box[2] = {box_cols, box_rows};
+  return make_tmap_nd(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, base, 2, dims, strides, box, true);
 }
 
 }  // namespace egovlp

@@ -210,6 +210,29 @@ __device__ __forceinline__ void tma_load_2d_multicast(uint32_t dst, const CUtens
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
+// 1-D bulk copy global -> smem (16B-aligned addresses, bytes % 16 == 0), completion on an mbarrier
+__device__ __forceinline__ void bulk_load_1d(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(dst), "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(bar)
+               : "memory");
+}
+// TMA store smem -> global (rows / columns outside the tensor are clipped), tracked by the issuing thread's bulk groups
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, uint32_t src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(src), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's bulk groups still READ their smem source (the buffers of the others may be rewritten)
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// at most N of this thread's bulk groups are incomplete (their global writes included)
+template <int N>
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+// barrier over `count` threads (a multiple of 32) on hardware barrier `id` (0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
 
 // ------------------------------------------------------------------------------------------
 // thread-block clusters
@@ -266,6 +289,9 @@ __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr, uint32_
 // 128B swizzle (box_cols * 2 bytes must be 128).
 int make_tmap_2d_bf16(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows,
                       uint32_t box_cols);
+// the same for fp32 (box_cols * 4 bytes must be 128)
+int make_tmap_2d_f32(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows,
+                     uint32_t box_cols);
 // Generic N-d (<=5) bf16 map: dims/strides innermost first, strides in elements (stride[0] must be 1).
 int make_tmap_nd_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides,
                       const uint32_t* box, bool swizzle128);

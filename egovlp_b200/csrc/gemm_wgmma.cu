@@ -16,13 +16,17 @@
 // TWO = CTA pair: a cluster of 2 CTAs computes a 256 x BLOCK_N tile; each CTA loads its own 128 rows of A and HALF of
 // the B tile, which TMA multicasts into both CTAs, so every B byte fetched from L2 feeds two SMs.  A stage is refilled
 // only once the math warpgroups of BOTH CTAs have released it (they arrive on the empty barriers of both).
-// Warp roles: warpgroup 0 = control (warp 0 lane 0 issues the TMA loads; warps 2 and 3 sum the A tiles' columns in the
-// wgrad form), warpgroups 1 and 2 = math: each issues m64 x BLOCK_N x k16 wgmmas for its 64 rows of the tile and then
-// runs the epilogue on its own accumulators, while the producer already streams the next tile's k-blocks into the
-// stages the math warpgroups have released.  setmaxnreg gives the control warpgroup 40 registers and the math
-// warpgroups 232 (BLOCK_N = 256 keeps 128 fp32 accumulators per thread).
+// Warp roles: warpgroup 0 = control (warp 0 lane 0 issues the TMA loads; warp 1 lane 0 loads the epilogue's inputs in
+// the specialised forms; warps 2 and 3 sum the A tiles' columns in the wgrad form), warpgroups 1 and 2 = math: each
+// issues m64 x BLOCK_N x k16 wgmmas for its 64 rows of the tile and then runs the epilogue on its own accumulators,
+// while the producer already streams the next tile's k-blocks into the stages the math warpgroups have released.
+// setmaxnreg gives the control warpgroup 40 registers and the math warpgroups 232 (BLOCK_N = 256 keeps 128 fp32
+// accumulators per thread).
 // The step's hot forms get compile-time specialised epilogues (EpiMode); the host picks the mode from the epilogue
-// descriptor, everything else takes the generic epilogue (same arithmetic, same order: bit-identical results).
+// descriptor, everything else takes the generic epilogue (same arithmetic, same order: bit-identical results).  The
+// specialised epilogues move their HBM bytes by TMA: the bias row and the residual / aux subtiles arrive in shared
+// memory while the tile's k-blocks run, and the results leave through 128B-swizzled staging subtiles as TMA stores that
+// drain while the math warpgroups already run the next tile.  The generic epilogue loads and stores from registers.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -57,12 +61,24 @@ struct EpiParams {
                     // gradient of the Linear whose weight gradient this GEMM computes, from the A tiles already in smem
 };
 
+// Specialised epilogues stage through shared memory: each math warpgroup owns EPI_BUFS subtiles of 64 rows x 128 B
+// (64 bf16 or 32 fp32 columns, 128B-swizzled like the operand tiles), which TMA fills with the residual / aux and
+// drains to the outputs; plus one fp32 bias row of the tile, shared by both warpgroups.
+constexpr int EPI_ROWS = 64;
+constexpr int EPI_SUB_BYTES = EPI_ROWS * 128;
+constexpr int EPI_BUFS = 2;
+constexpr int EPI_BIAS_BYTES = 256 * 4;
+constexpr int EPI_SMEM_BYTES = 2 * EPI_BUFS * EPI_SUB_BYTES + EPI_BIAS_BYTES;
+
 template <int BLOCK_N>
 struct Cfg {
   static constexpr int B_STAGE_BYTES = BLOCK_N * BLOCK_K * 2;
   static constexpr int STAGES = BLOCK_N == 256 ? 4 : 6;
   static constexpr int ACC = BLOCK_N / 2;     // fp32 accumulators per math thread (m64 x BLOCK_N over 128 threads)
-  static constexpr int SMEM_BYTES = STAGES * (A_STAGE_BYTES + B_STAGE_BYTES) + 1024 /*align*/ + 256 /*barriers*/;
+  static constexpr int RING_BYTES = STAGES * (A_STAGE_BYTES + B_STAGE_BYTES);
+  static constexpr int SMEM_BYTES = RING_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+  static constexpr int SMEM_BYTES_STAGED = SMEM_BYTES + EPI_SMEM_BYTES;
+  static_assert(SMEM_BYTES_STAGED <= 232448, "shared memory per block");
 };
 
 __device__ __forceinline__ void red_add_v4(float* p, float a, float b, float c, float d) {
@@ -208,8 +224,10 @@ enum EpiMode {
 
 template <int BLOCK_N, bool A_MN, bool B_MN, bool TWO, int MODE>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M, int N,
-                       int K, int num_m_blocks, int num_n_blocks, int kb_per_split, int num_splits, EpiParams ep) {
+gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                       const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmOut2,
+                       const __grid_constant__ CUtensorMap tmIn, int M, int N, int K, int num_m_blocks,
+                       int num_n_blocks, int kb_per_split, int num_splits, EpiParams ep) {
   static_assert(!(TWO && A_MN && B_MN), "the wgrad form (column sums of A) runs on single CTAs");
   using C = Cfg<BLOCK_N>;
   constexpr int TILE_M = TWO ? 2 * BLOCK_M : BLOCK_M;
@@ -217,13 +235,28 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
   const int worker = TWO ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
   const int num_workers = TWO ? (int)(gridDim.x >> 1) : (int)gridDim.x;
   constexpr int STAGES = C::STAGES;
+  // TMA-staged epilogue (the specialised forms): subtile width, subtiles per tile, which forms read an input subtile
+  // (the residual or aux, transformed in place) and which write two outputs (GELU and GELU', one buffer each)
+  constexpr bool STAGED = MODE != EPI_GENERIC;
+  constexpr bool OUT_F32 = MODE == EPI_RES_F32;
+  constexpr bool HAS_IN = MODE == EPI_RES_F32 || MODE == EPI_MUL_AUX;
+  constexpr bool TWO_OUT = MODE == EPI_ACT3;
+  constexpr int SUB_COLS = OUT_F32 ? 32 : 64;
+  constexpr int NSUB = BLOCK_N / SUB_COLS;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t sA = smem_base;
   const uint32_t sB = smem_base + STAGES * A_STAGE_BYTES;
-  const uint32_t bars = sB + STAGES * C::B_STAGE_BYTES;
+  const uint32_t sEpi = sB + STAGES * C::B_STAGE_BYTES;      // STAGED only: 2 warpgroups x EPI_BUFS subtiles
+  const uint32_t sBias = sEpi + 2 * EPI_BUFS * EPI_SUB_BYTES;
+  const uint32_t bars = STAGED ? sBias + EPI_BIAS_BYTES : sEpi;
   const uint32_t full_bar = bars;                    // STAGES x 8B
   const uint32_t empty_bar = bars + 8 * STAGES;      // STAGES x 8B
+  // STAGED: input subtile landed / subtile buffer free again ([warpgroup][buffer]), bias row landed / consumed
+  const uint32_t epi_full = bars + 16 * STAGES;
+  const uint32_t epi_empty = epi_full + 8 * 2 * EPI_BUFS;
+  const uint32_t bias_full = epi_empty + 8 * 2 * EPI_BUFS;
+  const uint32_t bias_empty = bias_full + 8;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -241,8 +274,21 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       // the two summing warps
       mbar_init(empty_bar + 8 * s, (TWO || sum_a) ? 4 : 2);
     }
+    if (STAGED) {
+      tma_prefetch_desc(&tmOut);
+      if (TWO_OUT) tma_prefetch_desc(&tmOut2);
+      if (HAS_IN) tma_prefetch_desc(&tmIn);
+      for (int i = 0; i < 2 * EPI_BUFS; ++i) {
+        mbar_init(epi_full + 8 * i, 1);
+        mbar_init(epi_empty + 8 * i, 1);      // the storing thread of the warpgroup, once its store has read the buffer
+      }
+      mbar_init(bias_full, 1);
+      mbar_init(bias_empty, 2);               // one arrive per math warpgroup
+    }
     fence_mbar_init();
   }
+  if (STAGED && !ep.bias && threadIdx.x < BLOCK_N)      // no bias: the row stays zero and is never loaded
+    asm volatile("st.shared.f32 [%0], %1;" ::"r"(sBias + 4 * threadIdx.x), "f"(0.f) : "memory");
   if (TWO) cluster_sync_all();      // the peer's barriers are initialised before any multicast or remote arrive
   else __syncthreads();
 
@@ -340,6 +386,39 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
           red_add_v4(ep.colsum_a + col + 4, acc[4], acc[5], acc[6], acc[7]);
         }
       }
+    } else if (STAGED && warp == 1) {
+      // ===================== epilogue inputs (TMA), while the math warpgroups run the tile's k-blocks =====================
+      // Per tile: the bias row once the previous tile's epilogue has consumed it, then the residual / aux subtiles of
+      // both warpgroups into their buffer rings as the stores of earlier subtiles free them.  Rows >= M and columns >= N
+      // are zero-filled by TMA.
+      if (lane == 0) {
+        uint32_t it = 0, tc = 0;
+        for (int unit = worker; unit < num_units; unit += num_workers, ++tc) {
+          const int m_blk = unit / num_n_blocks, n_blk = unit - m_blk * num_n_blocks;      // num_splits == 1
+          const int m_row = m_blk * TILE_M + (int)rank * BLOCK_M, n0 = n_blk * BLOCK_N;
+          mbar_wait_nocall(bias_empty, (tc & 1) ^ 1);
+          if (ep.bias) {
+            const uint32_t bytes = 4u * (uint32_t)min(BLOCK_N, N - n0);
+            mbar_expect_tx(bias_full, bytes);
+            bulk_load_1d(sBias, ep.bias + n0, bytes, bias_full);
+          } else {
+            mbar_arrive(bias_full);
+          }
+          if (HAS_IN) {
+            for (int s = 0; s < NSUB; ++s, ++it) {
+              const uint32_t b = it % EPI_BUFS, ph = (it / EPI_BUFS) & 1;
+#pragma unroll
+              for (int w = 0; w < 2; ++w) {
+                const uint32_t slot = w * EPI_BUFS + b;
+                mbar_wait_nocall(epi_empty + 8 * slot, ph ^ 1);
+                mbar_expect_tx(epi_full + 8 * slot, EPI_SUB_BYTES);
+                tma_load_2d(sEpi + slot * EPI_SUB_BYTES, &tmIn, epi_full + 8 * slot, n0 + s * SUB_COLS,
+                            m_row + w * EPI_ROWS);
+              }
+            }
+          }
+        }
+      }
     }
   } else {
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
@@ -353,20 +432,12 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
     };
     const int wq = warp & 3;                       // warp within the warpgroup: 16 accumulator rows each
     const GeluConsts gc;
-    constexpr bool GEN = MODE == EPI_GENERIC;
-    const int e_act = GEN ? ep.act : (MODE == EPI_ACT3 ? 3 : MODE == EPI_MUL_AUX ? 4 : MODE == EPI_ACT1 ? 1 : 0);
-    const int e_out_mode = GEN ? ep.out_mode : (MODE == EPI_RES_F32 ? 1 : 0);
-    const float* e_residual = (GEN || MODE == EPI_RES_F32) ? ep.residual : nullptr;
-    const bf16* e_aux = (GEN || MODE == EPI_MUL_AUX) ? ep.aux : nullptr;
-    float* e_colsum = GEN ? ep.colsum : nullptr;
-    bf16* e_out2 = (GEN || MODE == EPI_ACT3) ? ep.out2 : nullptr;
-    const int e_col_scale_ncols = (GEN || MODE == EPI_BF16) ? ep.col_scale_ncols : 0;
-    const int e_res_row_mod = GEN ? ep.res_row_mod : 0;
 
     float acc[C::ACC];
     int stage = 0;
     uint32_t phase = 0;
-    for (int unit = worker; unit < num_units; unit += num_workers) {
+    uint32_t it = 0, tc = 0;                       // STAGED: subtile and tile counters (ring / bias parities)
+    for (int unit = worker; unit < num_units; unit += num_workers, ++tc) {
       const int split = unit / num_tiles, tile = unit - split * num_tiles;
       const int m_blk = tile / num_n_blocks, n_blk = tile - m_blk * num_n_blocks;
       const int kb0 = split * kb_per_split, kb1 = min(num_kb, kb0 + kb_per_split);
@@ -399,6 +470,71 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
 
       // ---- epilogue.  Accumulator layout of m64nN: thread (warp wq, lane) holds rows wq*16 + lane/4 (+8) and, for
       // every 8-column group j, columns 8 j + 2 (lane % 4) + {0, 1}: acc[4 j + 2 h + {0, 1}] for row half h.
+      if constexpr (STAGED) {
+        // Subtile by subtile (64 rows x SUB_COLS): wait for the input subtile (HAS_IN), transform it -- or fill the
+        // buffer -- in place, fence to the async proxy, sync the warpgroup; then the leader stores the subtile by TMA
+        // (rows >= M / columns >= N clipped) and waits only until the store has READ the buffer before it is handed
+        // back to the input warp (or rewritten).  The global writes drain while the next subtile / tile runs.
+        const int m_row = m_blk * TILE_M + (int)rank * BLOCK_M + mw * EPI_ROWS, n0 = n_blk * BLOCK_N;
+        const int c2 = 2 * (lane & 3);
+        mbar_wait_nocall(bias_full, tc & 1);
+#pragma unroll
+        for (int s = 0; s < NSUB; ++s, ++it) {
+          const uint32_t b = it % EPI_BUFS, ph = (it / EPI_BUFS) & 1;
+          // two outputs fill both buffers: the previous subtile's stores must have read them (the leader waited)
+          if (TWO_OUT) named_bar_sync(1 + mw, 128);
+          const uint32_t buf = sEpi + (mw * EPI_BUFS + (TWO_OUT ? 0u : b)) * EPI_SUB_BYTES;
+          if (HAS_IN) mbar_wait_nocall(epi_full + 8 * (mw * EPI_BUFS + b), ph);
+#pragma unroll
+          for (int jj = 0; jj < SUB_COLS / 8; ++jj) {
+            const int j = s * (SUB_COLS / 8) + jj;        // 8-column group of the tile: constant after unrolling
+            float2 bq;
+            asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(bq.x), "=f"(bq.y) : "r"(sBias + 4 * (8 * j + c2)));
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int r = wq * 16 + (lane >> 2) + 8 * h;  // row of the subtile; 16-byte chunks XOR-swizzled by r & 7
+              // bf16: chunk jj, 4 bytes per lane pair; fp32: chunk 2 jj + (lane % 4) / 2, 8 bytes per lane pair
+              const uint32_t off = OUT_F32 ? r * 128 + (((2 * jj + ((lane & 3) >> 1)) ^ (r & 7)) << 4) + 8 * (lane & 1)
+                                           : r * 128 + ((jj ^ (r & 7)) << 4) + 4 * (lane & 3);
+              float v0 = __fmaf_rn(acc[4 * j + 2 * h], ep.alpha, bq.x);
+              float v1 = __fmaf_rn(acc[4 * j + 2 * h + 1], ep.alpha, bq.y);
+              if (MODE == EPI_BF16 && n0 + 8 * j + c2 < ep.col_scale_ncols) {
+                v0 = __fmul_rn(v0, ep.col_scale); v1 = __fmul_rn(v1, ep.col_scale);
+              }
+              if (MODE == EPI_ACT3) {           // out = GELU(v), out2 = GELU'(v)
+                uint32_t g, d;
+                gelu_and_grad2(gc, v0, v1, g, d);
+                asm volatile("st.shared.u32 [%0], %1;" ::"r"(buf + off), "r"(g) : "memory");
+                asm volatile("st.shared.u32 [%0], %1;" ::"r"(buf + EPI_SUB_BYTES + off), "r"(d) : "memory");
+              } else if (MODE == EPI_RES_F32) {
+                float r0, r1;
+                asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(r0), "=f"(r1) : "r"(buf + off) : "memory");
+                v0 += r0; v1 += r1;
+                asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(buf + off), "f"(v0), "f"(v1) : "memory");
+              } else {
+                if (MODE == EPI_ACT1) gelu2(gc, v0, v1);
+                if (MODE == EPI_MUL_AUX) {
+                  uint32_t a;
+                  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(a) : "r"(buf + off) : "memory");
+                  const float2 af = unpack_bf16x2(a);
+                  v0 *= af.x; v1 *= af.y;
+                }
+                asm volatile("st.shared.u32 [%0], %1;" ::"r"(buf + off), "r"(pack_bf16x2(v0, v1)) : "memory");
+              }
+            }
+          }
+          fence_proxy_async_smem();
+          named_bar_sync(1 + mw, 128);
+          if (leader) {
+            tma_store_2d(&tmOut, buf, n0 + s * SUB_COLS, m_row);
+            if (TWO_OUT) tma_store_2d(&tmOut2, buf + EPI_SUB_BYTES, n0 + s * SUB_COLS, m_row);
+            bulk_commit();
+            bulk_wait_read<0>();
+            if (HAS_IN) mbar_arrive(epi_empty + 8 * (mw * EPI_BUFS + b));
+          }
+        }
+        if (leader) mbar_arrive(bias_empty);      // after the last subtile's warpgroup sync: the bias row is read
+      } else {
       const int row_lo = m_blk * TILE_M + (int)rank * BLOCK_M + mw * 64 + wq * 16 + (lane >> 2);
       const int col_base = n_blk * BLOCK_N + 2 * (lane & 3);
 #pragma unroll
@@ -414,50 +550,52 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
           const bool rv = row < M;
           float v0 = __fmaf_rn(acc[4 * j + 2 * h], ep.alpha, bq.x);
           float v1 = __fmaf_rn(acc[4 * j + 2 * h + 1], ep.alpha, bq.y);
-          if (col < e_col_scale_ncols) { v0 = __fmul_rn(v0, ep.col_scale); v1 = __fmul_rn(v1, ep.col_scale); }
-          if (e_act == 3) {                  // out = GELU(v), out2 = GELU'(v)
+          if (col < ep.col_scale_ncols) { v0 = __fmul_rn(v0, ep.col_scale); v1 = __fmul_rn(v1, ep.col_scale); }
+          if (ep.act == 3) {                 // out = GELU(v), out2 = GELU'(v)
             uint32_t g, d;
             gelu_and_grad2(gc, v0, v1, g, d);
             if (rv) {
               *reinterpret_cast<uint32_t*>(reinterpret_cast<bf16*>(ep.out) + (long long)row * ep.ldo + col) = g;
-              if (e_out2) *reinterpret_cast<uint32_t*>(e_out2 + (long long)row * ep.ldo2 + col) = d;
+              if (ep.out2) *reinterpret_cast<uint32_t*>(ep.out2 + (long long)row * ep.ldo2 + col) = d;
             }
             continue;
           }
-          if (e_out2 && rv)                  // pre-activation (act 1) or a second copy
-            *reinterpret_cast<uint32_t*>(e_out2 + (long long)row * ep.ldo2 + col) = pack_bf16x2(v0, v1);
-          if (e_act == 1) gelu2(gc, v0, v1);
+          if (ep.out2 && rv)                 // pre-activation (act 1) or a second copy
+            *reinterpret_cast<uint32_t*>(ep.out2 + (long long)row * ep.ldo2 + col) = pack_bf16x2(v0, v1);
+          if (ep.act == 1) gelu2(gc, v0, v1);
           const int grow = rv ? row : M - 1;        // clamped: operand loads of padding rows stay in bounds
-          if (e_act == 2 || e_act == 4) {
-            const float2 a = unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(e_aux + (long long)grow * ep.ldaux + col)));
-            if (e_act == 2) { v0 *= gelu_grad_fast(a.x); v1 *= gelu_grad_fast(a.y); }
+          if (ep.act == 2 || ep.act == 4) {
+            const float2 a = unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(ep.aux + (long long)grow * ep.ldaux + col)));
+            if (ep.act == 2) { v0 *= gelu_grad_fast(a.x); v1 *= gelu_grad_fast(a.y); }
             else { v0 *= a.x; v1 *= a.y; }
           }
-          if (e_residual) {
-            const int rrow = e_res_row_mod ? grow % e_res_row_mod : grow;
-            const float2 r = __ldg(reinterpret_cast<const float2*>(e_residual + (long long)rrow * ep.ldr + col));
+          if (ep.residual) {
+            const int rrow = ep.res_row_mod ? grow % ep.res_row_mod : grow;
+            const float2 r = __ldg(reinterpret_cast<const float2*>(ep.residual + (long long)rrow * ep.ldr + col));
             v0 += r.x; v1 += r.y;
           }
           if (!rv) continue;
           cs0 += v0; cs1 += v1;
-          if (e_out_mode == 0) {
+          if (ep.out_mode == 0) {
             *reinterpret_cast<uint32_t*>(reinterpret_cast<bf16*>(ep.out) + (long long)row * ep.ldo + col) = pack_bf16x2(v0, v1);
-          } else if (e_out_mode == 1) {
+          } else if (ep.out_mode == 1) {
             *reinterpret_cast<float2*>(reinterpret_cast<float*>(ep.out) + (long long)row * ep.ldo + col) = make_float2(v0, v1);
           } else {
             red_add_v2(reinterpret_cast<float*>(ep.out) + (long long)row * ep.ldo + col, v0, v1);
           }
         }
-        if (e_colsum) {     // lanes with the same lane % 4 hold the same two columns: fold, then one atomic pair
+        if (ep.colsum) {    // lanes with the same lane % 4 hold the same two columns: fold, then one atomic pair
 #pragma unroll
           for (int o = 4; o < 32; o <<= 1) {
             cs0 += __shfl_xor_sync(0xffffffffu, cs0, o);
             cs1 += __shfl_xor_sync(0xffffffffu, cs1, o);
           }
-          if (lane < 4) red_add_v2(e_colsum + col, cs0, cs1);
+          if (lane < 4) red_add_v2(ep.colsum + col, cs0, cs1);
         }
       }
+      }
     }
+    if (STAGED && leader) bulk_wait<0>();      // this warpgroup's last stores are complete before the CTA exits
   }
   if (TWO) cluster_sync_all();      // the peer may still multicast into this CTA's smem or arrive on its barriers
 }
@@ -474,6 +612,19 @@ int launch(const void* A, long long lda, const void* B, long long ldb, int M, in
   if (!B_MN) rc = make_tmap_2d_bf16(&tmB, B, N, K, ldb, TWO ? BLOCK_N / 2 : BLOCK_N, BLOCK_K);
   else       rc = make_tmap_2d_bf16(&tmB, B, K, N, ldb, BLOCK_K, 64);
   if (rc) return rc;
+  // epilogue subtiles of the staged forms: [64 rows, 128 B] boxes over out / out2 / residual / aux
+  constexpr bool STAGED = MODE != EPI_GENERIC;
+  CUtensorMap tmOut = {}, tmOut2 = {}, tmIn = {};
+  if (MODE == EPI_RES_F32) {
+    rc = make_tmap_2d_f32(&tmOut, ep.out, M, N, ep.ldo, EPI_ROWS, 32);
+    if (!rc) rc = make_tmap_2d_f32(&tmIn, ep.residual, M, N, ep.ldr, EPI_ROWS, 32);
+  } else if (STAGED) {
+    rc = make_tmap_2d_bf16(&tmOut, ep.out, M, N, ep.ldo, EPI_ROWS, 64);
+    if (!rc && MODE == EPI_ACT3) rc = make_tmap_2d_bf16(&tmOut2, ep.out2, M, N, ep.ldo2, EPI_ROWS, 64);
+    if (!rc && MODE == EPI_MUL_AUX) rc = make_tmap_2d_bf16(&tmIn, ep.aux, M, N, ep.ldaux, EPI_ROWS, 64);
+  }
+  if (rc) return rc;
+  constexpr int SMEM_BYTES = STAGED ? C::SMEM_BYTES_STAGED : C::SMEM_BYTES;
   constexpr int TILE_M = TWO ? 2 * BLOCK_M : BLOCK_M;
   const int num_m_blocks = (M + TILE_M - 1) / TILE_M, num_n_blocks = (N + BLOCK_N - 1) / BLOCK_N;
   const int num_kb = (K + BLOCK_K - 1) / BLOCK_K;
@@ -484,13 +635,13 @@ int launch(const void* A, long long lda, const void* B, long long ldb, int M, in
   auto kern = gemm_bf16_wgmma_kernel<BLOCK_N, A_MN, B_MN, TWO, MODE>;
   static bool attr_set = false;
   if (!attr_set) {
-    EGOVLP_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
+    EGOVLP_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
     attr_set = true;
   }
   cudaLaunchConfig_t cfg = {};
   cudaLaunchAttribute attr[1];
   cfg.blockDim = dim3(NUM_THREADS);
-  cfg.dynamicSmemBytes = C::SMEM_BYTES;
+  cfg.dynamicSmemBytes = SMEM_BYTES;
   cfg.stream = stream;
   if (TWO) {
     attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -515,7 +666,8 @@ int launch(const void* A, long long lda, const void* B, long long ldb, int M, in
   }
   const int workers = min(units, resident);
   cfg.gridDim = dim3(TWO ? 2 * workers : workers);
-  EGOVLP_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, M, N, K, num_m_blocks, num_n_blocks, kb_per_split, splits, ep));
+  EGOVLP_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, tmOut, tmOut2, tmIn, M, N, K, num_m_blocks, num_n_blocks,
+                                       kb_per_split, splits, ep));
   return EGOVLP_OK;
 }
 
@@ -529,18 +681,30 @@ int dispatch_major(int a_mn, int b_mn, const void* A, long long lda, const void*
   return launch<BLOCK_N, true, false, false, EPI_GENERIC>(A, lda, B, ldb, M, N, K, splits, ep, stream);
 }
 
+// TMA's rules for a tensor the staged epilogue loads or stores: 16-byte aligned base, row stride a multiple of 16 bytes
+inline bool tma_ok(const void* p, long long ld_bytes) {
+  return (reinterpret_cast<uintptr_t>(p) & 15) == 0 && ld_bytes % 16 == 0;
+}
+
 // Which specialised epilogue (if any) computes exactly what `ep` asks for; EGOVLP_GEMM_GENERIC_EPI=1 keeps every call on
-// the generic one (the kernel tests run both and compare).
+// the generic one (the kernel tests run both and compare).  The specialised forms move their epilogue bytes by TMA, so a
+// call whose tensors TMA cannot address (see tma_ok; the bias row is a 1-D bulk copy) takes the generic epilogue.
 inline int epi_mode(const EpiParams& ep) {
   const char* g = getenv("EGOVLP_GEMM_GENERIC_EPI");
   if (g && g[0] == '1') return EPI_GENERIC;
   if (ep.colsum || ep.res_row_mod) return EPI_GENERIC;
+  if (ep.bias && (reinterpret_cast<uintptr_t>(ep.bias) & 15) != 0) return EPI_GENERIC;
   const bool no_scale = ep.col_scale_ncols == 0;
-  if (ep.act == 0 && ep.out_mode == 0 && !ep.residual && !ep.out2) return EPI_BF16;
-  if (ep.act == 3 && ep.out_mode == 0 && !ep.residual && ep.out2 && no_scale) return EPI_ACT3;
-  if (ep.act == 4 && ep.out_mode == 0 && !ep.residual && !ep.out2 && no_scale) return EPI_MUL_AUX;
-  if (ep.act == 0 && ep.out_mode == 1 && ep.residual && !ep.out2 && no_scale) return EPI_RES_F32;
-  if (ep.act == 1 && ep.out_mode == 0 && !ep.residual && !ep.out2 && no_scale) return EPI_ACT1;
+  const bool out16 = tma_ok(ep.out, ep.ldo * 2);
+  if (ep.act == 0 && ep.out_mode == 0 && !ep.residual && !ep.out2 && out16) return EPI_BF16;
+  if (ep.act == 3 && ep.out_mode == 0 && !ep.residual && ep.out2 && no_scale && out16 && tma_ok(ep.out2, ep.ldo2 * 2))
+    return EPI_ACT3;
+  if (ep.act == 4 && ep.out_mode == 0 && !ep.residual && !ep.out2 && no_scale && out16 && tma_ok(ep.aux, ep.ldaux * 2))
+    return EPI_MUL_AUX;
+  if (ep.act == 0 && ep.out_mode == 1 && ep.residual && !ep.out2 && no_scale && tma_ok(ep.out, ep.ldo * 4) &&
+      tma_ok(ep.residual, ep.ldr * 4))
+    return EPI_RES_F32;
+  if (ep.act == 1 && ep.out_mode == 0 && !ep.residual && !ep.out2 && no_scale && out16) return EPI_ACT1;
   return EPI_GENERIC;
 }
 

@@ -1,18 +1,39 @@
-"""Micro-benchmark of the wgmma GEMM on the shapes of the 16-frame step (B=64 -> M=200768 tokens)."""
+"""Per-form timing of the GEMM calls one video block (SpaceTimeBlockFn) makes at the headline step's size.
+
+    python tools/bench_gemm.py [--M 100384] [--iters 20] [--json out.json]
+
+cfg3 = 32 clips x (1 + 16 x 196) tokens = 100,384 rows.  Every call of engine.py's forward and input-gradient GEMMs is
+timed with CUDA events, with the same dtypes, epilogue arguments and b_mn flags, plus the weight gradients with
+engine._split_for's split.  A form that reads or writes more than one bf16 output's worth of epilogue bytes is also timed
+with the plain bf16 epilogue on the same A.B: the difference is what its epilogue costs on top.  Each specialised form is
+checked bit for bit against the generic epilogue (EGOVLP_GEMM_GENERIC_EPI=1) at this size.
+EGOVLP_B200_LIB=<path> runs another build of the library (A/B comparisons)."""
+import argparse
 import json
-import sys
 import os
+import subprocess
+import sys
+
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from egovlp_b200 import ops
+from egovlp_b200 import engine, ops  # noqa: E402
 
-M = int(os.environ.get("M", 200768))
-dev = "cuda"
-peaks = json.load(open("MEASURED_PEAKS.json")) if os.path.exists("MEASURED_PEAKS.json") else {"bf16_tflops": 1590.0}
+D, HID = 768, 3072
+BF16, F32 = torch.bfloat16, torch.float32
 
 
-def t(fn, iters=10):
+def gpu_info():
+    q = "name,power.limit,clocks.sm,clocks.max.sm"
+    try:
+        r = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True,
+                           timeout=30)
+        return r.stdout.strip().splitlines()[0] if r.returncode == 0 and r.stdout.strip() else "unavailable"
+    except (OSError, subprocess.TimeoutExpired):
+        return "unavailable"
+
+
+def timed(fn, iters):
     for _ in range(3):
         fn()
     torch.cuda.synchronize()
@@ -25,43 +46,110 @@ def t(fn, iters=10):
     return s.elapsed_time(e) / iters
 
 
-def rnd(*shape, dt=torch.bfloat16):
-    return (torch.randn(*shape, device=dev) * 0.05).to(dt)
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--M", type=int, default=32 * (1 + 16 * 196))
+    ap.add_argument("--iters", type=int, default=20)
+    ap.add_argument("--json", default=None)
+    args = ap.parse_args()
+    assert torch.cuda.is_available(), "bench_gemm.py measures on the GPU"
+    M, dev = args.M, "cuda"
+    g = torch.Generator(device=dev).manual_seed(0)
+
+    def rnd(*shape, dt=BF16, scale=0.05):
+        return (torch.randn(*shape, device=dev, generator=g) * scale).to(dt)
+
+    x768, x3072 = rnd(M, D, scale=1.0), rnd(M, HID, scale=1.0)
+    dy768, dy2304, dy3072 = rnd(M, D, scale=1.0), rnd(M, 3 * D, scale=1.0), rnd(M, HID, scale=1.0)
+    w_qkv, w_proj, w_fc1, w_fc2 = rnd(3 * D, D), rnd(D, D), rnd(HID, D), rnd(D, HID)
+    b_qkv, b_proj, b_fc1, b_fc2 = (rnd(n, dt=F32) for n in (3 * D, D, HID, D))
+    res = rnd(M, D, dt=F32, scale=1.0)
+    u = rnd(M, HID, scale=1.0)
+    sms = engine._sm_count(torch.cuda.current_device())
+
+    # (name, calls per block, A, B, out shape/dtype, gemm kwargs, epilogue HBM bytes, specialised)
+    def fwd(name, n, a, w, out_dt, kw, ebytes):
+        return (name, n, a, w, (M, w.shape[0]), out_dt, kw, ebytes, True)
+
+    def dgrad(name, n, a, w, out_dt, kw, ebytes):
+        return (name, n, a, w, (M, w.shape[1]), out_dt, dict(kw, b_mn=True), ebytes, True)
+
+    forms = [
+        fwd("qkv fwd (bias, q-scale -> bf16)", 2, x768, w_qkv, BF16,
+            dict(bias=b_qkv, col_scale=0.125, col_scale_ncols=D), M * 3 * D * 2),
+        fwd("proj fwd (bias + fp32 residual)", 2, x768, w_proj, F32, dict(bias=b_proj, residual=res), M * D * 8),
+        fwd("fc1 fwd (GELU, GELU')", 1, x768, w_fc1, BF16, dict(bias=b_fc1, act=3, out2="out2"), M * HID * 4),
+        fwd("fc2 fwd (bias + fp32 residual)", 1, x3072, w_fc2, F32, dict(bias=b_fc2, residual=res), M * D * 8),
+        dgrad("fc2 dgrad (x GELU')", 1, dy768, w_fc2, BF16, dict(aux=u, act=4), M * HID * 4),
+        dgrad("fc1 dgrad", 1, dy3072, w_fc1, BF16, {}, M * D * 2),
+        dgrad("proj dgrad", 2, dy768, w_proj, BF16, {}, M * D * 2),
+        dgrad("qkv dgrad", 2, dy2304, w_qkv, BF16, {}, M * D * 2),
+    ]
+    rows, report = [], {"gpu": gpu_info(), "M": M, "lib": os.environ.get("EGOVLP_B200_LIB") or "in-tree",
+                        "forms": []}
+    surcharge_block, ms_block, mismatches = 0.0, 0.0, []
+    for name, n, a, w, shape, out_dt, kw, ebytes, _ in forms:
+        out = torch.empty(*shape, device=dev, dtype=out_dt)
+        kw = dict(kw)
+        if kw.get("out2") == "out2":
+            kw["out2"] = torch.empty(*shape, device=dev, dtype=BF16)
+        call = lambda: ops.gemm(a, w, out, **kw)  # noqa: E731
+        ms = timed(call, args.iters)
+        flop = 2.0 * M * shape[1] * a.shape[1]
+        plain_ms = None
+        if ebytes > M * shape[1] * 2:
+            o16 = torch.empty(*shape, device=dev, dtype=BF16)
+            plain = dict(b_mn=True) if kw.get("b_mn") else {}
+            plain_ms = timed(lambda: ops.gemm(a, w, o16, **plain), args.iters)
+            surcharge_block += n * (ms - plain_ms)
+        ms_block += n * ms
+        # bit-identical to the generic epilogue at this size
+        os.environ["EGOVLP_GEMM_GENERIC_EPI"] = "1"
+        call()
+        ref = [out.clone()] + ([kw["out2"].clone()] if "out2" in kw else [])
+        os.environ["EGOVLP_GEMM_GENERIC_EPI"] = "0"
+        out.fill_(float("nan"))
+        call()
+        got = [out] + ([kw["out2"]] if "out2" in kw else [])
+        same = all(torch.equal(r, q) for r, q in zip(ref, got))
+        if not same:
+            mismatches.append(name)
+        rows.append((name, n, ms, flop / ms / 1e9, ebytes / 1e6, plain_ms, same))
+        report["forms"].append(dict(name=name, calls_per_block=n, ms=ms, tflops=flop / ms / 1e9, epilogue_mb=ebytes / 1e6,
+                                    plain_bf16_ms=plain_ms, bitwise_equal_generic=same))
+    os.environ.pop("EGOVLP_GEMM_GENERIC_EPI", None)
+    # weight gradients (split-K fp32 atomics, generic epilogue), the engine's split rule
+    for name, n, dy, x, n_out, n_in, colsum in [("fc2 wgrad", 1, dy768, x3072, D, HID, False),
+                                                ("fc1 wgrad (+ bias grad)", 1, dy3072, x768, HID, D, True),
+                                                ("proj wgrad", 2, dy768, x768, D, D, False),
+                                                ("qkv wgrad (+ bias grad)", 2, dy2304, x768, 3 * D, D, True)]:
+        split = engine._split_for(n_out, n_in, M, sms)
+        dw = torch.zeros(n_out, n_in, device=dev, dtype=F32)
+        db = torch.zeros(n_out, device=dev, dtype=F32) if colsum else None
+        ms = timed(lambda: ops.gemm(dy, x, dw, a_mn=True, b_mn=True, accumulate=True, split_k=split, colsum_a=db),
+                   args.iters)
+        flop = 2.0 * M * n_out * n_in
+        ms_block += n * ms
+        rows.append((f"{name} split {split}", n, ms, flop / ms / 1e9, n_out * n_in * 4 / 1e6, None, None))
+        report["forms"].append(dict(name=name, split=split, calls_per_block=n, ms=ms, tflops=flop / ms / 1e9))
+
+    print(f"GPU: {report['gpu']}   (name, power limit, SM clock, max SM clock)")
+    print(f"M = {M}, library: {report['lib']}")
+    print(f"{'form':40s} {'x/blk':>5s} {'ms':>8s} {'TFLOP/s':>8s} {'epi MB':>8s} {'plain ms':>9s} {'surcharge':>9s}  bitwise")
+    for name, n, ms, tf, mb, plain_ms, same in rows:
+        pl = f"{plain_ms:9.3f}" if plain_ms is not None else " " * 9
+        sc = f"{ms - plain_ms:9.3f}" if plain_ms is not None else " " * 9
+        eq = "" if same is None else ("yes" if same else "NO")
+        print(f"{name:40s} {n:5d} {ms:8.3f} {tf:8.1f} {mb:8.1f} {pl} {sc}  {eq}")
+    print(f"per block: GEMMs {ms_block:.3f} ms, epilogue surcharge {surcharge_block:.3f} ms; "
+          f"x 12 blocks: {12 * ms_block:.1f} ms, surcharge {12 * surcharge_block:.1f} ms")
+    report.update(block_ms=ms_block, block_surcharge_ms=surcharge_block, mismatches=mismatches)
+    if args.json:
+        with open(args.json, "w") as f:
+            json.dump(report, f, indent=1)
+    if mismatches:
+        sys.exit(f"specialised epilogue differs from the generic one: {mismatches}")
 
 
-rows = []
-for name, N, K in [("qkv", 2304, 768), ("proj", 768, 768), ("fc1", 3072, 768), ("fc2", 768, 3072)]:
-    a, w = rnd(M, K), rnd(N, K)
-    bias = rnd(N, dt=torch.float32)
-    out = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
-    ms = t(lambda: ops.gemm(a, w, out, bias=bias))
-    ref = t(lambda: torch.nn.functional.linear(a, w, bias.to(torch.bfloat16)))
-    fl = 2.0 * M * N * K
-    rows.append((f"fwd {name} bias", ms, fl / ms / 1e9, ref))
-    if name == "fc1":
-        u = torch.empty_like(out)
-        ms = t(lambda: ops.gemm(a, w, out, bias=bias, act=1, out2=u))
-        rows.append((f"fwd {name} bias+gelu+preact", ms, fl / ms / 1e9, ref))
-    if name in ("proj", "fc2"):
-        res = rnd(M, N, dt=torch.float32)
-        o32 = torch.empty(M, N, device=dev, dtype=torch.float32)
-        ms = t(lambda: ops.gemm(a, w, o32, bias=bias, residual=res))
-        rows.append((f"fwd {name} bias+res->f32", ms, fl / ms / 1e9, ref))
-    # dgrad: dx[M,K] = dy[M,N] @ W[N,K]
-    dy = rnd(M, N)
-    dx = torch.empty(M, K, device=dev, dtype=torch.float32 if name != "fc2" else torch.bfloat16)
-    ms = t(lambda: ops.gemm(dy, w, dx, b_mn=True))
-    ref = t(lambda: torch.matmul(dy, w))
-    rows.append((f"dgrad {name}", ms, fl / ms / 1e9, ref))
-    # wgrad: dW[N,K] += dy^T a
-    dw = torch.zeros(N, K, device=dev, dtype=torch.float32)
-    for split in (4, 8, 16):
-        ms = t(lambda: ops.gemm(dy, a, dw, a_mn=True, b_mn=True, accumulate=True, split_k=split))
-        rows.append((f"wgrad {name} split{split}", ms, fl / ms / 1e9, None))
-    ref = t(lambda: torch.matmul(dy.t(), a))
-    rows[-1] = rows[-1][:3] + (ref,)
-
-print(f"M={M}  peak(burst)={peaks['bf16_tflops']} TF/s")
-for name, ms, tf, ref in rows:
-    extra = f"  cublas {ref:.3f} ms" if ref else ""
-    print(f"{name:32s} {ms:8.3f} ms  {tf:8.1f} TF/s  {tf / peaks['bf16_tflops'] * 100:5.1f}%{extra}")
+if __name__ == "__main__":
+    main()
