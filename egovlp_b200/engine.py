@@ -317,13 +317,16 @@ class PatchEmbedFn(torch.autograd.Function):
         B, T, N, D, K, F = ctx.dims
         dx = dx.contiguous().view(-1, D)
         dx16 = _bf16_of(dx)
-        dw = wgrad(dx16, patches, D, K)
+        if K % 32 == 0:
+            dw = wgrad(dx16, patches, D, K)
+        else:           # the GEMM's N must be a multiple of 32 (K = 432 at P = 12): form dW^T = patches^T dx instead
+            dw = wgrad(patches, dx16, K, D).t()
         dcls, dpos = _zeros((1, 1, D), dx), _zeros((1, N + 1, D), dx)
         dtemp, dbias = _zeros((1, F, D), dx), _zeros((D,), dx)
         tmp = _empty(((1 + T * N) * D,), F32, dx)
         ops.video_embed_bwd(dx, tmp, dcls, dpos, dtemp, dbias, B, T, N, D)
         P = int(round((K // 3) ** 0.5))
-        return None, dcls, dpos, dtemp, dw.view(D, 3, P, P), dbias, None, None
+        return None, dcls, dpos, dtemp, dw.reshape(D, 3, P, P), dbias, None, None
 
 
 class SpaceTimeBlockFn(torch.autograd.Function):

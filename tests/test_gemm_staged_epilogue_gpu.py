@@ -26,40 +26,88 @@ def mk(shape, seed, scale=1.0, dtype=torch.bfloat16):
 
 
 def rel_err(a, b):
-    return ((a.float() - b.float()).norm() / b.float().norm().clamp_min(1e-30)).item()
+    return ((a.double() - b.double()).norm() / b.double().norm().clamp_min(1e-30)).item()
 
 
 def run_forms(ops, a, b, wt, bias, res, aux):
+    """Every specialised epilogue form -- bias -> bf16 (BF16), GELU + GELU' (ACT3), x aux (MUL_AUX), bias + fp32
+    residual (RES_F32), GELU (ACT1) -- first with K-major B (`b`, [N, K]), then with MN-major B (`wt`, [K, N]): ten
+    calls, twelve outputs, in the order of `references`."""
     M, N = a.shape[0], b.shape[0]
     outs = []
-    o = torch.full((M, N), 7.0, device="cuda", dtype=torch.bfloat16)
-    ops.gemm(a, b, o, bias=bias, col_scale=0.125, col_scale_ncols=min(N, 64)); outs.append(o)
-    o = torch.full((M, N), 7.0, device="cuda", dtype=torch.bfloat16)
-    ops.gemm(a, wt, o, b_mn=True); outs.append(o)
-    h, d = torch.empty(M, N, device="cuda", dtype=torch.bfloat16), torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
-    ops.gemm(a, b, h, bias=bias, act=3, out2=d); outs += [h, d]
-    o = torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
-    ops.gemm(a, wt, o, b_mn=True, aux=aux, act=4); outs.append(o)
-    o = torch.empty(M, N, device="cuda", dtype=torch.float32)
-    ops.gemm(a, b, o, bias=bias, residual=res); outs.append(o)
-    o = torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
-    ops.gemm(a, b, o, bias=None, act=1); outs.append(o)
+    for bb, b_mn in ((b, False), (wt, True)):
+        o = torch.full((M, N), 7.0, device="cuda", dtype=torch.bfloat16)
+        if b_mn:
+            ops.gemm(a, bb, o, b_mn=True); outs.append(o)
+        else:
+            ops.gemm(a, bb, o, bias=bias, col_scale=0.125, col_scale_ncols=min(N, 64)); outs.append(o)
+        h, d = torch.empty(M, N, device="cuda", dtype=torch.bfloat16), torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
+        ops.gemm(a, bb, h, b_mn=b_mn, bias=bias, act=3, out2=d); outs += [h, d]
+        o = torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
+        ops.gemm(a, bb, o, b_mn=b_mn, aux=aux, act=4); outs.append(o)
+        o = torch.empty(M, N, device="cuda", dtype=torch.float32)
+        ops.gemm(a, bb, o, b_mn=b_mn, bias=bias, residual=res); outs.append(o)
+        o = torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
+        ops.gemm(a, bb, o, b_mn=b_mn, bias=None, act=1); outs.append(o)
     torch.cuda.synchronize()
     return outs
 
 
-@pytest.mark.parametrize("M,N,K", [(70, 256, 64), (333, 384, 192), (129, 96, 64), (517, 512, 128)])
+def references(a, b, bias, res, aux):
+    """fp64 values of the twelve outputs of `run_forms` (its MN-major B is b^T, so both halves share one product)."""
+    N = b.shape[0]
+    acc = a.double() @ b.double().t()
+    accb = acc + bias.double()
+    scaled = accb.clone()
+    scaled[:, :min(N, 64)] *= 0.125
+    x = accb.clone().requires_grad_(True)
+    gelu = torch.nn.functional.gelu(x)
+    gelu.sum().backward()
+    rest = [gelu.detach(), x.grad, acc * aux.double(), accb + res.double(), torch.nn.functional.gelu(acc)]
+    return [scaled] + rest + [acc] + rest
+
+
+# M ragged for a warpgroup's or a whole CTA's rows; N = 384 runs 128-column tiles and N = 512 256-column ones (CTA pairs
+# under the fixture); K = 72 and 200 end in a partial k-block that TMA zero-fills
+@pytest.mark.parametrize("M,N,K", [(70, 256, 64), (333, 384, 192), (129, 96, 64), (517, 512, 128), (190, 256, 72),
+                                   (301, 384, 200)])
 def test_staged_epilogues_match_the_generic_one_on_ragged_shapes(ops, monkeypatch, gemm_mode, M, N, K):
-    """Rows past M (a warpgroup's or a whole CTA's rows), N % 128 != 0 (partial 64-column subtiles), no bias."""
-    a, b, wt = mk((M, K), 40), mk((N, K), 41, 0.06), mk((K, N), 42, 0.06)
+    """All ten (form, B layout) pairs: bit for bit against the generic epilogue and within the GEMM tolerances of fp64
+    (bf16 outputs rel-L2 4e-3, fp32 outputs 2e-5).  Rows past M, N % 128 != 0 (partial 64-column subtiles), no bias."""
+    a, b = mk((M, K), 40), mk((N, K), 41, 0.06)
+    wt = b.t().contiguous()
     bias, res, aux = mk((N,), 43, dtype=torch.float32), mk((M, N), 44, dtype=torch.float32), mk((M, N), 45)
     monkeypatch.setenv("EGOVLP_GEMM_GENERIC_EPI", "1")
     ref = run_forms(ops, a, b, wt, bias, res, aux)
     monkeypatch.setenv("EGOVLP_GEMM_GENERIC_EPI", "0")
     got = run_forms(ops, a, b, wt, bias, res, aux)
-    for i, (r, g) in enumerate(zip(ref, got)):
+    assert len(got) == 12
+    for i, (r, g, want) in enumerate(zip(ref, got, references(a, b, bias, res, aux))):
         assert torch.equal(r, g), i
-    assert rel_err(got[5], a.float() @ b.float().t() + bias + res) < 2e-5
+        tol = 2e-5 if g.dtype == torch.float32 else 4e-3
+        assert rel_err(g, want) < tol, (i, rel_err(g, want))
+
+
+@pytest.mark.parametrize("K", [2304, 3072])
+@pytest.mark.parametrize("M", [117, 512])
+def test_residual_f32_with_mn_major_b_at_text_backward_shapes(ops, monkeypatch, gemm_mode, M, K):
+    """dx = dy @ W + fp32 residual with W stored [K, N]: the text tower's backward runs it twice per layer (the lin1
+    input gradient plus the residual path, K = 3072, and the q|k|v input gradient plus the attention branch, K = 2304)."""
+    N = 768
+    a, w, res = mk((M, K), 70), mk((K, N), 71, 0.03), mk((M, N), 72, dtype=torch.float32)
+
+    def run():
+        o = torch.full((M, N), float("nan"), device="cuda", dtype=torch.float32)
+        ops.gemm(a, w, o, b_mn=True, residual=res)
+        torch.cuda.synchronize()
+        return o
+
+    monkeypatch.setenv("EGOVLP_GEMM_GENERIC_EPI", "1")
+    ref = run()
+    monkeypatch.setenv("EGOVLP_GEMM_GENERIC_EPI", "0")
+    got = run()
+    assert torch.equal(ref, got)
+    assert rel_err(got, a.double() @ w.double() + res.double()) < 2e-5
 
 
 def test_staged_epilogue_writes_only_its_view(ops, gemm_mode):
