@@ -258,6 +258,77 @@ __global__ void egomcq_kernel(const float* __restrict__ text, const float* __res
   if (lane == 0) pred[q] = besti;
 }
 
+// Softmax cross-entropy (model/loss.py:135-141 = nn.CrossEntropyLoss() with its defaults: mean over the rows whose
+// target is not ignore_index, no class weights, no label smoothing).  One warp per row: max-subtracted log-sum-exp,
+// row loss = lse - x[target]; 0 on an ignored row, NaN for a target outside [0, C) (never used as an index).
+__device__ __forceinline__ bool ce_bad_target(long long t, int C, int ignore) { return t != ignore && (t < 0 || t >= C); }
+
+__global__ void ce_rows_kernel(const float* __restrict__ x, long long ld, const long long* __restrict__ target, int G,
+                               int C, int ignore, float* __restrict__ lse, float* __restrict__ row_loss) {
+  const int r = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (r >= G) return;
+  const float* xr = x + (long long)r * ld;
+  float mx = -INFINITY;
+  for (int c = lane; c < C; c += 32) mx = fmaxf(mx, xr[c]);
+  mx = warp_max(mx);
+  float s = 0.f;
+  for (int c = lane; c < C; c += 32) s += expf(xr[c] - mx);
+  s = warp_sum(s);
+  if (lane == 0) {
+    const float l = mx + logf(s);
+    const long long t = target[r];
+    lse[r] = l;
+    row_loss[r] = t == ignore ? 0.f : ce_bad_target(t, C, ignore) ? NAN : l - xr[t];
+  }
+}
+// out[0] = sum(row_loss) / n_valid, out[1] = n_valid (as float): ONE CTA, each thread sums a fixed stride of rows, then a
+// fixed butterfly / shared-memory tree, so the loss is bitwise reproducible.  n_valid = 0 gives 0 / 0 = NaN, as torch.
+__global__ void __launch_bounds__(1024)
+ce_reduce_kernel(const float* __restrict__ row_loss, const long long* __restrict__ target, int G, int ignore,
+                 float* __restrict__ out) {
+  __shared__ float rs[32];
+  __shared__ int rn[32];
+  float s = 0.f;
+  int n = 0;
+  for (int i = threadIdx.x; i < G; i += blockDim.x) {
+    s += row_loss[i];
+    n += target[i] != ignore;
+  }
+  s = warp_sum(s);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) n += __shfl_xor_sync(0xffffffffu, n, o);
+  if ((threadIdx.x & 31) == 0) { rs[threadIdx.x >> 5] = s; rn[threadIdx.x >> 5] = n; }
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    const bool have = threadIdx.x < (blockDim.x >> 5);
+    s = warp_sum(have ? rs[threadIdx.x] : 0.f);
+    n = have ? rn[threadIdx.x] : 0;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) n += __shfl_xor_sync(0xffffffffu, n, o);
+    if (threadIdx.x == 0) {
+      out[0] = s / (float)n;
+      out[1] = (float)n;
+    }
+  }
+}
+// dx[r, c] = g * (softmax(x_r)_c - [c == target_r]) / n_valid; 0 on ignored rows, NaN on rows with a bad target
+__global__ void ce_bwd_kernel(const float* __restrict__ x, long long ld, const long long* __restrict__ target,
+                              const float* __restrict__ lse, const float* __restrict__ out, int G, int C, int ignore,
+                              const float* __restrict__ gscale, float* __restrict__ dx) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long long)G * C) return;
+  const int r = idx / C, c = idx % C;
+  const long long t = target[r];
+  float v;
+  if (t == ignore) v = 0.f;
+  else if (ce_bad_target(t, C, ignore)) v = NAN;
+  else {
+    const float p = expf(x[(long long)r * ld + c] - lse[r]);
+    v = (gscale ? *gscale : 1.f) * (p - (c == t ? 1.f : 0.f)) / out[1];
+  }
+  dx[idx] = v;
+}
+
 }  // namespace
 }  // namespace egovlp
 
@@ -362,6 +433,28 @@ extern "C" int egovlp_egomcq_score(const float* text, const float* video, float*
   EGOVLP_CHECK_ARG(text && video && scores && pred && Q >= 0 && K > 0 && C > 0, "egomcq_score: bad args");
   if (Q == 0) return EGOVLP_OK;
   egomcq_kernel<<<(Q + 7) / 8, 256, 0, ST(stream)>>>(text, video, scores, pred, Q, K, C, eps);
+  EGOVLP_CHECK_LAUNCH();
+  return EGOVLP_OK;
+}
+extern "C" int egovlp_cross_entropy_fwd(const float* logits, long long ld, const long long* target, int G, int C,
+                                        int ignore_index, float* lse, float* row_loss, float* out, void* stream) {
+  EGOVLP_CHECK_ARG(logits && target && lse && row_loss && out && G >= 0 && C > 0 && ld >= C, "cross_entropy_fwd: bad args");
+  if (G > 0) {
+    ce_rows_kernel<<<(G + 7) / 8, 256, 0, ST(stream)>>>(logits, ld, target, G, C, ignore_index, lse, row_loss);
+    EGOVLP_CHECK_LAUNCH();
+  }
+  ce_reduce_kernel<<<1, 1024, 0, ST(stream)>>>(row_loss, target, G, ignore_index, out);
+  EGOVLP_CHECK_LAUNCH();
+  return EGOVLP_OK;
+}
+extern "C" int egovlp_cross_entropy_bwd(const float* logits, long long ld, const long long* target, const float* lse,
+                                        const float* out, int G, int C, int ignore_index, const float* gscale, float* dx,
+                                        void* stream) {
+  EGOVLP_CHECK_ARG(logits && target && lse && out && dx && G >= 0 && C > 0 && ld >= C, "cross_entropy_bwd: bad args");
+  const long long n = (long long)G * C;
+  if (n == 0) return EGOVLP_OK;
+  ce_bwd_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ST(stream)>>>(logits, ld, target, lse, out, G, C, ignore_index,
+                                                                    gscale, dx);
   EGOVLP_CHECK_LAUNCH();
   return EGOVLP_OK;
 }

@@ -281,6 +281,27 @@ def bgrad(dy):
     return db
 
 
+def _linear_fwd(act16, w16, b, out):
+    """out = act16 w16^T + b for the projection heads (model/model.py:72-79): the wgmma GEMM, or for the widths it cannot
+    take (C % 32 != 0, e.g. the OSCC / PNR fine-tuning heads of width 2 / 16) the narrow-head kernels."""
+    if w16.shape[0] % 32:
+        ops.narrow_linear_fwd(act16, w16, b, out)
+    else:
+        ops.gemm(act16, w16, out, bias=b)
+
+
+def _linear_bwd(dout, act16, w16):
+    """-> (dW, db, d_act fp32) of `_linear_fwd` from its fp32 output gradient; both products take d16 = bf16(dout)."""
+    n_out, n_in = w16.shape
+    d16 = ops.cast_bf16(dout)
+    if n_out % 32:
+        return ops.narrow_linear_bwd(dout, d16, act16, w16)
+    g_w, g_b = wgrad(d16, act16, n_out, n_in), bgrad(dout)
+    dact = _empty((act16.shape[0], n_in), F32, dout)
+    ops.gemm(d16, w16, dact, b_mn=True)
+    return g_w, g_b, dact
+
+
 # ----------------------------------------------------------------------------------------------------------
 # video tower
 # ----------------------------------------------------------------------------------------------------------
@@ -469,7 +490,7 @@ class ClsHeadFn(torch.autograd.Function):
             ctx.save_for_backward(x, mean, rstd, nw)
             return y32
         out = _empty((B, pw.shape[0]), F32, x)
-        ops.gemm(y16, cache.get(pw), out, bias=pb.detach())
+        _linear_fwd(y16, cache.get(pw), pb.detach(), out)
         ctx.save_for_backward(x, mean, rstd, nw, y16, pw)
         return out
 
@@ -481,11 +502,7 @@ class ClsHeadFn(torch.autograd.Function):
         g_pw = g_pb = None
         if ctx.has_proj:
             x, mean, rstd, nw, y16, pw = ctx.saved_tensors
-            Pd = pw.shape[0]
-            d16 = ops.cast_bf16(dout)
-            g_pw, g_pb = wgrad(d16, y16, Pd, D), bgrad(dout)
-            dn = _empty((B, D), F32, dout)
-            ops.gemm(d16, ctx.cache.get(pw), dn, b_mn=True)
+            g_pw, g_pb, dn = _linear_bwd(dout, y16, ctx.cache.get(pw))
         else:
             x, mean, rstd, nw = ctx.saved_tensors
             dn = dout
@@ -574,7 +591,7 @@ class TextTowerFn(torch.autograd.Function):
             r16 = _empty((rows, D), BF16, dev)
             ops.relu_rows_fwd(x, stride, r16, rows, D)
             out = _empty((rows, pw.shape[0]), F32, dev)
-            ops.gemm(r16, cache.get(pw), out, bias=pb.detach())
+            _linear_fwd(r16, cache.get(pw), pb.detach(), out)
         if train:
             ctx.meta = (B, L, D, heads, tokens_mode, len(layers), len(saved), p_hid, p_att, seed)
             ctx.cache = cache
@@ -598,10 +615,7 @@ class TextTowerFn(torch.autograd.Function):
             pw, pb = p[-2:]
             Pd = pw.shape[0]
             dout = dout.contiguous().float().view(rows, Pd)
-            d16 = ops.cast_bf16(dout)
-            g_pw, g_pb = wgrad(d16, r16, Pd, D), bgrad(dout)
-            dr = _empty((rows, D), F32, dout)
-            ops.gemm(d16, cache.get(pw), dr, b_mn=True)
+            g_pw, g_pb, dr = _linear_bwd(dout, r16, cache.get(pw))
             dx = _zeros((M, D), dout)
             ops.relu_rows_bwd(x_last, stride, dr, dx, rows, D)
         else:
@@ -771,3 +785,23 @@ class MaxMarginFn(torch.autograd.Function):
         x = ctx.saved_tensors[0]
         w = ctx.saved_tensors[1] if ctx.has_w else None
         return ops.maxmargin_bwd(x, ctx.args[0], ctx.args[1], g.contiguous().float(), w), None, None, None
+
+
+class CrossEntropyFn(torch.autograd.Function):
+    """nn.CrossEntropyLoss() with its defaults (model/loss.py:135-141): mean over the rows whose target is not
+    `ignore_index` of the max-subtracted LSE minus the target logit, fp32.  `x` [G, C] is read in place when its rows are
+    unit-stride."""
+
+    @staticmethod
+    def forward(ctx, x, target, ignore_index):
+        x = x if (x.dtype == F32 and x.stride(1) == 1) else x.float().contiguous()
+        target = target.contiguous()
+        loss, lse, stats = ops.cross_entropy_fwd(x, target, ignore_index)
+        ctx.ignore_index = ignore_index
+        ctx.save_for_backward(x, target, lse, stats)
+        return loss
+
+    @staticmethod
+    def backward(ctx, g):
+        x, target, lse, stats = ctx.saved_tensors
+        return ops.cross_entropy_bwd(x, target, lse, stats, g.contiguous().float(), ctx.ignore_index), None, None

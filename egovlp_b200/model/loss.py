@@ -1,5 +1,6 @@
 """Losses of the reference's model/loss.py on CUDA kernels: same class names, constructor arguments and
-forward signatures.  CrossEntropy (OSCC / PNR heads) is outside the hot-path scope (SURVEY.md 2)."""
+forward signatures -- the contrastive losses of pretraining / EPIC-MIR and the CrossEntropy of the Ego4D OSCC / PNR
+fine-tuning heads."""
 import torch
 from torch import nn
 
@@ -77,3 +78,19 @@ class AdaptiveMaxMarginRankingLoss(nn.Module):
         if weight is None:
             raise AttributeError("AdaptiveMaxMarginRankingLoss needs `weight` [n] (the reference calls weight.unsqueeze)")
         return engine.MaxMarginFn.apply(x, self.margin, self.fix_norm, weight)
+
+
+class CrossEntropy(nn.Module):
+    """model/loss.py:135-141: nn.CrossEntropyLoss() with its defaults (mean over the rows whose target is not -100, no
+    class weights, no label smoothing) on the cross-entropy kernels.  The reference's callers
+    (trainer/trainer_oscc.py:337, trainer/trainer_pnr.py:348) pass [G, C] logits and int64 class indices; other target
+    forms (class probabilities, extra dimensions) are not implemented.  A class index outside [0, C) gives a NaN loss
+    where torch raises a device assert."""
+
+    ignore_index = -100
+
+    def forward(self, output, target):
+        if output.dim() != 2 or target.dim() != 1 or target.dtype != torch.int64 or target.shape[0] != output.shape[0]:
+            raise NotImplementedError(f"CrossEntropy: [G, C] logits and int64 class indices [G] expected, got "
+                                      f"{tuple(output.shape)} {output.dtype} and {tuple(target.shape)} {target.dtype}")
+        return engine.CrossEntropyFn.apply(output, target.to(output.device), self.ignore_index)

@@ -1,4 +1,8 @@
-"""EgoMCQ metric of the reference's model/metric.py (:218-234) with GPU scoring (ops.egomcq_score)."""
+"""Metrics of the reference's model/metric.py: EgoMCQ (:218-234) with GPU scoring (ops.egomcq_score), EPIC-MIR
+(:236-299) and the Ego4D OSCC / PNR fine-tuning metrics (:342-397)."""
+import warnings
+
+import numpy as np
 import torch
 
 from .. import ops
@@ -79,3 +83,42 @@ def mir_metrics(similarity_matrix, idx_arr):
     with open(os.path.join(base, "relevancy/caption_relevancy_EPIC_100_retrieval_test.pkl"), "rb") as f:
         relevancy = pickle.load(f)
     return mir_metrics_core(similarity_matrix, idx_arr, video_id, text_id, relevancy)
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# Ego4D hand-object benchmarks (model/metric.py:342-397)
+# ------------------------------------------------------------------------------------------------------------------
+
+def _rows_argmax(preds):
+    """argmax of every row (flattened), ties -> lowest index: torch.argmax(pred) per row as the reference loops do."""
+    preds = torch.as_tensor(preds)
+    return torch.argmax(preds.reshape(preds.shape[0], -1), dim=1)
+
+
+def oscc_metrics(preds, labels):
+    """model/metric.py:342-353: accuracy in % of the row-wise argmax of `preds` [N, C] against `labels` [N]."""
+    pred = _rows_argmax(preds)
+    correct = (pred == torch.as_tensor(labels).to(pred.device).reshape(-1)).sum().item()
+    return {"accuracy": correct / pred.shape[0] * 100}
+
+
+def pnr_metrics(preds, labels, sc_labels, fps, parent_start_frames, parent_end_frames, parent_pnr_frames):
+    """model/metric.py:355-397: mean keyframe error in seconds over the clips with a state change (`sc_labels == 1`).
+    The predicted keyframe maps to `(parent_end - parent_start) / 16 * argmax`, a true division of the frame tensors
+    (float32 for integer frame numbers, as in the reference); the error is |mapped - (pnr - start)| / fps in float64.
+    No state-change clip gives NaN: the reference's `np.mean(0.0)` fallback (:388-393) is overwritten by
+    `np.mean([])` on the next line."""
+    pred = _rows_argmax(preds)
+    dev = pred.device
+
+    def col(v):
+        return torch.as_tensor(v).to(dev).reshape(-1)
+
+    sc, start, end, pnr, rate = (col(v) for v in (sc_labels, parent_start_frames, parent_end_frames,
+                                                  parent_pnr_frames, fps))
+    keep = sc == 1
+    mapped = (end[keep] - start[keep]) / 16 * pred[keep]
+    err = (mapped.double() - (pnr[keep].double() - start[keep].double())).abs() / rate[keep].double()
+    with warnings.catch_warnings(), np.errstate(invalid="ignore"):
+        warnings.simplefilter("ignore", RuntimeWarning)
+        return {"keyframe_distance": np.mean(err.cpu().numpy())}

@@ -281,6 +281,39 @@ def relu_rows_bwd(x, row_stride, dh, dx, rows, D):
     call("egovlp_relu_rows_bwd", _ptr(x), C.c_longlong(row_stride), _ptr(dh), _ptr(dx), rows, D, _stream())
 
 
+# ---------------------------------------------------------------- narrow projection heads (C % 32 != 0)
+def narrow_linear_fwd(act16, w16, bias, out):
+    """out fp32 [rows, C] = act16 [rows, K] @ w16 [C, K]^T + bias (fp32 [C])."""
+    _chk(act16, BF16, "act16"); _chk(w16, BF16, "w16"); _chk(out, F32, "out")
+    rows, K = act16.shape
+    Cc = w16.shape[0]
+    assert act16.is_contiguous() and w16.is_contiguous() and w16.shape == (Cc, K)
+    assert out.is_contiguous() and out.shape == (rows, Cc)
+    if bias is not None:
+        _chk(bias, F32, "bias"); assert bias.is_contiguous() and bias.numel() == Cc
+    call("egovlp_narrow_linear_fwd", _ptr(act16), _ptr(w16), _ptr(bias), _ptr(out), rows, Cc, K, _stream())
+    return out
+
+
+def narrow_linear_bwd(dout, d16, act16, w16):
+    """-> (dW fp32 [C, K] = d16^T act16, db fp32 [C] = colsum(dout), d_act fp32 [rows, K] = d16 w16)."""
+    _chk(dout, F32, "dout"); _chk(d16, BF16, "d16"); _chk(act16, BF16, "act16"); _chk(w16, BF16, "w16")
+    rows, K = act16.shape
+    Cc = w16.shape[0]
+    for t in (dout, d16, act16, w16):
+        assert t.is_contiguous()
+    assert dout.shape == (rows, Cc) and d16.shape == (rows, Cc) and w16.shape == (Cc, K)
+    dev = act16.device
+    dw = torch.empty(Cc, K, dtype=F32, device=dev)
+    db = torch.empty(Cc, dtype=F32, device=dev)
+    dact = torch.empty(rows, K, dtype=F32, device=dev)
+    n_ws = lib().egovlp_narrow_linear_workspace_floats(rows, Cc, K)
+    ws = torch.empty(n_ws, dtype=F32, device=dev) if n_ws > 0 else None
+    call("egovlp_narrow_linear_bwd", _ptr(dout), _ptr(d16), _ptr(act16), _ptr(w16), _ptr(dw), _ptr(db), _ptr(dact),
+         _ptr(ws), rows, Cc, K, _stream())
+    return dw, db, dact
+
+
 # ---------------------------------------------------------------- similarity / losses (fp32)
 def rownorm_fwd(a, eps=1e-8):
     _chk(a, F32, "a")
@@ -436,6 +469,29 @@ def maxmargin_bwd(x, margin, fix_norm, gscale, row_weight=None):
     dx = torch.empty_like(x)
     call("egovlp_maxmargin_bwd", _ptr(x), _ptr(row_weight), x.shape[0], C.c_float(margin), int(fix_norm), _ptr(gscale),
          _ptr(dx), _stream())
+    return dx
+
+
+def cross_entropy_fwd(x, target, ignore_index=-100):
+    """x fp32 [G, C] (row stride free), target int64 [G] -> (loss fp32 scalar, lse fp32 [G], stats fp32 [2] =
+    (loss, n_valid))."""
+    x = _rows_view(x, "logits")
+    assert target.is_cuda and target.dtype == torch.int64 and target.is_contiguous() and target.shape == (x.shape[0],)
+    G, Cc = x.shape
+    lse = torch.empty(G, dtype=F32, device=x.device)
+    row_loss = torch.empty(G, dtype=F32, device=x.device)
+    stats = torch.empty(2, dtype=F32, device=x.device)
+    call("egovlp_cross_entropy_fwd", _ptr(x), C.c_longlong(x.stride(0) if G > 0 else Cc), _ptr(target), G, Cc,
+         int(ignore_index), _ptr(lse), _ptr(row_loss), _ptr(stats), _stream())
+    return stats[0], lse, stats
+
+
+def cross_entropy_bwd(x, target, lse, stats, gscale, ignore_index=-100):
+    """-> dx fp32 [G, C] = gscale * (softmax(x) - onehot(target)) / n_valid (0 on ignored rows)."""
+    G, Cc = x.shape
+    dx = torch.empty(G, Cc, dtype=F32, device=x.device)
+    call("egovlp_cross_entropy_bwd", _ptr(x), C.c_longlong(x.stride(0) if G > 0 else Cc), _ptr(target), _ptr(lse),
+         _ptr(stats), G, Cc, int(ignore_index), _ptr(gscale), _ptr(dx), _stream())
     return dx
 
 

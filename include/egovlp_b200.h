@@ -162,6 +162,22 @@ int egovlp_relu_rows_fwd(const float* x, long long row_stride, void* out_bf16, i
 int egovlp_relu_rows_bwd(const float* x, long long row_stride, const float* dh, float* dx, int rows, int D, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Narrow projection heads: the vid_proj / txt_proj Linear(K, C) of model/model.py:72-79 for widths C the GEMM above
+ * cannot take (C % 32 != 0: the OSCC head C = 2, configs/ft/oscc.json; the PNR head C = 16, configs/ft/pnr.json).
+ * CUDA-core kernels, no atomics: bitwise reproducible.  All tensors contiguous; K % 8 == 0, 16B-aligned bases.
+ *   fwd: out fp32 [rows, C] = act bf16 [rows, K] . w bf16 [C, K]^T + bias fp32 [C] (bias may be NULL); K <= 2048.
+ *   bwd: from dout_bf16 [rows, C] (= bf16(dout)):  dw fp32 [C, K] = dout_bf16^T . act,  dact fp32 [rows, K] =
+ *        dout_bf16 . w  (rows <= 65535), and from the fp32 dout [rows, C]: db fp32 [C] = column sums of dout.  Each of
+ *        dw / db / dact may be NULL.  dw needs a workspace of egovlp_narrow_linear_workspace_floats(rows, C, K) floats
+ *        (0: none) for its row splits, which are merged in a fixed order.
+ */
+int egovlp_narrow_linear_fwd(const void* act_bf16, const void* w_bf16, const float* bias, float* out, int rows, int C,
+                             int K, void* stream);
+long long egovlp_narrow_linear_workspace_floats(int rows, int C, int K);
+int egovlp_narrow_linear_bwd(const float* dout, const void* dout_bf16, const void* act_bf16, const void* w_bf16,
+                             float* dw, float* db, float* dact, float* workspace, int rows, int C, int K, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Similarity and losses, fp32 (model/model.py:189-197 sim_matrix; model/loss.py EgoNCE :34-53,
  * NormSoftmaxLoss :13-25, MaxMarginRankingLoss :63-90; run/test_epic.py:137-143 dual softmax;
  * trainer/trainer_egoclip.py:204-215 + model/metric.py:227 EgoMCQ scoring).
@@ -220,6 +236,20 @@ int egovlp_egonce_fused_bwd(const float* text, long long ld_t, const float* vide
                             float* d_text, float* d_video, void* stream);
 int egovlp_egomcq_score(const float* text, const float* video, float* scores, long long* pred, int Q, int K, int C,
                         float eps, void* stream);
+
+/* Softmax cross-entropy, nn.CrossEntropyLoss() with its defaults (model/loss.py:135-141; the OSCC / PNR fine-tuning
+ * steps, trainer/trainer_oscc.py:333-338, trainer/trainer_pnr.py:341-348).  logits fp32 [G, C] (row stride ld),
+ * target int64 [G].  Forward: lse fp32 [G] (max-subtracted log-sum-exp per row), row_loss fp32 [G] (workspace),
+ * out fp32 [2] = {mean of lse - logit[target] over the rows whose target != ignore_index, number of those rows}.
+ * A target outside [0, C) that is not ignore_index is never used as an index: its row loss, hence the loss, is NaN
+ * (torch raises a device assert instead).  No valid row gives 0 / 0 = NaN, as torch.  The reduction order is fixed:
+ * the loss is bitwise reproducible.  Backward: dx fp32 [G, C] contiguous = gscale[0] * (softmax - onehot) / n_valid,
+ * zero on ignored rows, NaN on rows with a bad target (gscale device pointer or NULL for 1). */
+int egovlp_cross_entropy_fwd(const float* logits, long long ld, const long long* target, int G, int C, int ignore_index,
+                             float* lse, float* row_loss, float* out, void* stream);
+int egovlp_cross_entropy_bwd(const float* logits, long long ld, const long long* target, const float* lse,
+                             const float* out, int G, int C, int ignore_index, const float* gscale, float* dx,
+                             void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Retrieval evaluation (EPIC-Kitchens MIR; SURVEY.md 8f row 3).  Replaces the host numpy argsort + fancy indexing of
