@@ -1,11 +1,74 @@
-"""Metrics of the reference's model/metric.py: EgoMCQ (:218-234) with GPU scoring (ops.egomcq_score), EPIC-MIR
-(:236-299) and the Ego4D OSCC / PNR fine-tuning metrics (:342-397)."""
+"""Metrics of the reference's model/metric.py: the t2v / v2t retrieval ranks (:20-216) on the GPU (ops.gt_ranks),
+EgoMCQ (:218-234) with GPU scoring (ops.egomcq_score), EPIC-MIR (:236-299), Charades-Ego mAP (:301-340) on the ranking
+kernel and the Ego4D OSCC / PNR fine-tuning metrics (:342-397)."""
 import warnings
 
 import numpy as np
 import torch
 
 from .. import ops
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# MSR-VTT-style retrieval ranks (model/metric.py:20-216; the NLQ / MQ evaluation configs list them)
+# ------------------------------------------------------------------------------------------------------------------
+
+def _sims_dev(sims):
+    from ..utils.nDCG import _dev
+    s = _dev(sims)
+    return s if s.dtype in (torch.float32, torch.float64) else s.double()
+
+
+def _host(x):
+    return x.detach().cpu().numpy() if isinstance(x, torch.Tensor) else np.asarray(x)
+
+
+def cols2metrics(cols, num_queries):
+    """The rank vector -> metrics, as Frozen-in-Time defines it (the reference calls it but never defines it): R@k =
+    100 * #(rank < k) / num_queries for k in 1, 5, 10, 50; MedR / MeanR = median / mean of the ranks + 1; and the
+    geometric mean of R1, R5, R10."""
+    import scipy.stats                  # only here: the other metrics of this module do not need scipy
+    cols = _host(cols)
+    metrics = {}
+    for k in (1, 5, 10, 50):
+        metrics[f"R{k}"] = 100 * float(np.sum(cols < k)) / num_queries
+    metrics["MedR"] = np.median(cols) + 1
+    metrics["MeanR"] = np.mean(cols) + 1
+    stats = [metrics[x] for x in ("R1", "R5", "R10")]
+    with warnings.catch_warnings():
+        warnings.simplefilter("ignore", RuntimeWarning)         # log(0) of an R@k of 0, as scipy reports it
+        metrics["geometric_mean_R1-R5-R10"] = scipy.stats.mstats.gmean(stats)
+    return metrics
+
+
+def t2v_ranks(sims, query_masks=None):
+    """0-based rank of every (kept) query's ground-truth video: sims [Q, V], ground truth of query i is video
+    i // (Q // V), ties broken optimistically.  -> (fp64 ranks on the device, number of queries)."""
+    ranks = ops.gt_ranks(_sims_dev(sims), 0)
+    if query_masks is None:
+        return ranks, ranks.shape[0]
+    keep = torch.as_tensor(_host(query_masks).reshape(-1).astype(bool))
+    assert keep.numel() == ranks.shape[0], "invalid query mask shape"
+    return ranks[keep.to(ranks.device)], int(keep.sum())
+
+
+def v2t_ranks(sims, query_masks=None):
+    """0-based rank of every video's closest ground-truth caption: sims [N, V] (text x video, transposed here as the
+    reference does), captions [i c, (i + 1) c) of video i with c = N // V, ties averaged; query_masks [N] marks
+    missing captions.  -> (fp64 ranks on the device, number of videos)."""
+    s = _sims_dev(sims).t().contiguous()
+    mask = None if query_masks is None else torch.as_tensor((_host(query_masks).reshape(-1) != 0).astype(np.uint8))
+    return ops.gt_ranks(s, 1, mask), s.shape[0]
+
+
+def t2v_metrics(sims, query_masks=None):
+    """model/metric.py:20-124 (numpy or torch input, moved to the current CUDA device)."""
+    return cols2metrics(*t2v_ranks(sims, query_masks))
+
+
+def v2t_metrics(sims, query_masks=None):
+    """model/metric.py:127-216 (numpy or torch input, moved to the current CUDA device)."""
+    return cols2metrics(*v2t_ranks(sims, query_masks))
 
 
 def egomcq_predict(text_embeds, video_embeds):
@@ -83,6 +146,36 @@ def mir_metrics(similarity_matrix, idx_arr):
     with open(os.path.join(base, "relevancy/caption_relevancy_EPIC_100_retrieval_test.pkl"), "rb") as f:
         relevancy = pickle.load(f)
     return mir_metrics_core(similarity_matrix, idx_arr, video_id, text_id, relevancy)
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# Charades-Ego (model/metric.py:301-340)
+# ------------------------------------------------------------------------------------------------------------------
+
+CHARADES_MAX_VIDEOS = 16384          # egovlp_rank_metrics ranks at most this many items per query (one CTA in smem)
+
+
+def charades_class_ap(submission_array, gt_array):
+    """Average precision of every class of a [videos, classes] score matrix (fp64 [classes] on the device): videos
+    whose ground truth is empty score -inf; within a class, videos rank by score (compared in fp32), equal scores by
+    smaller video index first, NaN scores after every real one as numpy's argsort of -score puts them; AP = sum of
+    precision@k over the true positives (gt == 1) / their number, NaN for a class without one."""
+    from ..utils.nDCG import _dev
+    sub = _dev(submission_array, torch.float32)
+    gt = _dev(gt_array)
+    assert sub.dim() == 2 and gt.shape == sub.shape, "expected [videos, classes] scores and targets"
+    if sub.shape[0] > CHARADES_MAX_VIDEOS:
+        raise ValueError(f"charades_metrics: {sub.shape[0]} videos, at most {CHARADES_MAX_VIDEOS} are supported")
+    empty = gt.sum(dim=1) == 0
+    fix = torch.where(empty[:, None], torch.full_like(sub, -float("inf")), sub)
+    _, ap = ops.rank_metrics(fix.t().contiguous(), (gt == 1).t().float().contiguous(), tie_mode=0, want_dcg=False)
+    return ap
+
+
+def charades_metrics(submission_array, gt_array):
+    """model/metric.py:327-340: {'mAP': mean class AP} as a fraction; a class without a positive makes it NaN."""
+    ap = charades_class_ap(submission_array, gt_array).cpu().numpy()
+    return {"mAP": np.mean(ap)}
 
 
 # ------------------------------------------------------------------------------------------------------------------

@@ -191,5 +191,13 @@ class FrozenInTime(BaseModel):
 
 
 def sim_matrix(a, b, eps=1e-8):
-    """Cosine similarity a_n @ b_n^T with norms clamped at eps (reference model/model.py:189-197)."""
+    """Cosine similarity a_n @ b_n^T with norms clamped at eps (reference model/model.py:189-197).  Host tensors (the
+    reference's evaluation loops move embeddings to the host first) are computed on the current CUDA device and the
+    result comes back to the host; the copies are ordinary `.to()` calls, so autograd sees them.  Without CUDA this
+    raises, like every other op of the package."""
+    if a.device != b.device:
+        raise RuntimeError(f"sim_matrix: expected both inputs on the same device, got {a.device} and {b.device}")
+    if a.device.type == "cpu" and torch.cuda.is_available():
+        dev = torch.device("cuda", torch.cuda.current_device())
+        return engine.SimMatrixFn.apply(a.to(dev), b.to(dev), eps).to(a.device)
     return engine.SimMatrixFn.apply(a, b, eps)

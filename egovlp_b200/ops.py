@@ -514,6 +514,23 @@ def rank_metrics(sim, rel, k_counts=None, tie_mode=0, want_dcg=True, want_ap=Tru
     return dcg, ap
 
 
+def gt_ranks(sims, mode, col_mask=None):
+    """Ground-truth ranks (egovlp_gt_ranks): sims fp32/fp64 [rows, cols] on CUDA -> fp64 [rows], 0-based.  mode 0 (t2v):
+    [queries, videos], ties optimistic; mode 1 (v2t): [videos, captions], ties averaged, min over each video's captions,
+    col_mask [captions] (0 = missing caption).  Synchronises; raises EgovlpError on a NaN row or an invalid shape."""
+    assert sims.is_cuda and sims.dtype in (torch.float32, torch.float64) and sims.dim() == 2
+    sims = sims if sims.stride(1) == 1 else sims.contiguous()
+    rows, cols = sims.shape
+    if col_mask is not None:
+        assert mode == 1 and col_mask.numel() == cols
+        col_mask = col_mask.reshape(-1).to(device=sims.device, dtype=torch.uint8).contiguous()
+    ranks = torch.empty(rows, dtype=torch.float64, device=sims.device)
+    status = torch.empty(1, dtype=torch.int32, device=sims.device)
+    call("egovlp_gt_ranks", _ptr(sims), int(sims.dtype == torch.float64), C.c_longlong(sims.stride(0)), rows, cols,
+         int(mode), _ptr(col_mask), _ptr(ranks), _ptr(status), _stream())
+    return ranks
+
+
 def dual_softmax(sim, temp=500.0):
     _chk(sim, F32, "sim")
     sim = sim.contiguous()

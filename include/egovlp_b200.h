@@ -260,11 +260,31 @@ int egovlp_cross_entropy_bwd(const float* logits, long long ld, const long long*
  *            calculate_k_counts, nDCG.py:47-75, produces)
  *   tie_mode 0: equal similarities rank by smaller column first (stable argsort of -sim, mAP.py:25);
  *            1: by larger column first (stable ascending argsort reversed, nDCG.py:32)
+ *            NaN similarities rank where numpy's sort puts them: after every real value (-inf included) in mode 0,
+ *            before every real value in mode 1, among themselves by the same column rule.
  *   dcg[row] = sum_i k_i * rel[row, rank_i] / log2(i + 2);  ap[row] = sum_i [rel_i == 1] cumsum(rel)_i / (i + 1) / #(rel == 1)
  *            (NaN for a row without relevant items, as numpy).  Either output may be NULL.  cols <= 16384.
  */
 int egovlp_rank_metrics(const float* sim, long long ld_sim, const void* rel, int rel_is_f64, long long ld_rel,
                         const int* k_counts, int rows, int cols, int tie_mode, double* dcg, double* ap, void* stream);
+
+/* Ground-truth ranks of the MSR-VTT-style retrieval metrics (model/metric.py:20-216, t2v_metrics / v2t_metrics), which
+ * rank by distance subtraction, so their ranks are fully determined, ties included.  One CTA counts, per candidate, the
+ * entries of its row with a greater and with an equal similarity; no sort.  sims fp32 or fp64 [rows, cols] (row stride
+ * ld), compared exactly in that type.  ranks fp64 [rows], 0-based.
+ *   mode 0 (t2v): rows = queries, cols = videos, rows % cols == 0, q = rows / cols; row i's ground truth is column i / q;
+ *                 rank = #{j : sims[i, j] > sims[i, gt]} (ties optimistic).  col_mask must be NULL.
+ *   mode 1 (v2t): rows = videos, cols = captions (sims transposed), c = cols / rows (floor) <= egovlp_gt_ranks_max_candidates();
+ *                 candidates of row i are columns [i c, (i + 1) c); per candidate rank = #greater + (#equal - 1) / 2
+ *                 (ties averaged); the row's rank is the minimum over its candidates, +inf if none is left.  col_mask
+ *                 uint8 [cols] or NULL: entries with col_mask == 0 become similarity -1e8 (the reference's distance
+ *                 MISSING_VAL); candidates equal to -1e8 or non-finite are skipped.
+ * status: int [1] device workspace (bits: 1 NaN in a row, 2 non-finite t2v ground truth).  The call SYNCHRONISES the
+ * stream to read it and returns EGOVLP_ERR_ARG, naming every condition found, for a NaN anywhere in a row (after the
+ * caption mask) or (t2v) a non-finite ground-truth similarity.  cols <= 65535 * 256. */
+int egovlp_gt_ranks_max_candidates(void);
+int egovlp_gt_ranks(const void* sims, int is_f64, long long ld, int rows, int cols, int mode, const uint8_t* col_mask,
+                    double* ranks, int* status, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Elementwise / reduction helpers on the path.
