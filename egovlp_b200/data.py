@@ -27,10 +27,12 @@ def _record(obj, stream):
 
 
 class DevicePrefetcher:
-    """Iterates `loader` (batches of pinned host tensors / nested dicts) one batch ahead on a copy stream."""
+    """Iterates `loader` (batches of pinned host tensors / nested dicts) one batch ahead on a copy stream.
+    `transform`, if given, is called on each batch on the copy stream after its H2D copy (e.g.
+    `transforms.DeviceVideoTransform`, which turns packed uint8 clips into the model's fp32 frames)."""
 
-    def __init__(self, loader, device):
-        self.loader, self.device = loader, torch.device(device)
+    def __init__(self, loader, device, transform=None):
+        self.loader, self.device, self.transform = loader, torch.device(device), transform
         self.stream = torch.cuda.Stream(device=self.device)
 
     def __iter__(self):
@@ -49,4 +51,5 @@ class DevicePrefetcher:
         except StopIteration:
             return None
         with torch.cuda.stream(self.stream):
-            return _to_device(batch, self.device)
+            batch = _to_device(batch, self.device)
+            return batch if self.transform is None else self.transform(batch)

@@ -233,6 +233,60 @@ def patch_im2col_u8(video, patches, P, mean, std):
     call("egovlp_patch_im2col_u8", _ptr(video), _ptr(patches), B, T, Cc, H, W, P, m3, s3, _stream())
 
 
+def video_transform(frames, desc, F, R, center_crop, mean, std):
+    """Dataset video transforms on the GPU (egovlp_video_transform): frames = packed uint8 clips on CUDA (clip b is
+    [T, H, W, 3] at byte offset desc[b, 0]); desc = host int64 [B, 10] rows (offset, T, H, W, mode, i, j, h, w, flip),
+    mode 0 = train (crop box + flip), 1 = eval.  Returns fp32 [B, F, 3, R, R]; frames t >= T are 0.0.  The table is
+    checked here, before launch: a row the kernel would have to refuse raises EgovlpError."""
+    import numpy as np
+    from ._lib import EgovlpError
+    _chk(frames, torch.uint8, "frames")
+    assert frames.dim() == 1 and frames.is_contiguous()
+    d = np.asarray(desc.numpy() if torch.is_tensor(desc) else desc)
+    if d.ndim != 2 or d.shape[1] != 10 or d.shape[0] < 1 or d.dtype.kind not in "iu":
+        raise EgovlpError(f"video_transform: descriptor table must be integer [B >= 1, 10], got {d.dtype} {d.shape}")
+    d = d.astype(np.int64)
+    off, T, H, W, mode, i, j, h, w, flip = d.T
+    B = d.shape[0]
+    bad = []
+    def rows(mask, what):
+        if mask.any():
+            bad.append(f"{what} (clips {np.flatnonzero(mask)[:8].tolist()})")
+    rows((H < 1) | (W < 1) | (H > 65535) | (W > 65535), "frame size outside [1, 65535]")
+    rows((T < 1) | (T > F), f"frame count outside [1, F={F}]")
+    rows((mode != 0) & (mode != 1), "mode not 0 (train) or 1 (eval)")
+    ok = (H >= 1) & (W >= 1) & (H <= 65535) & (W <= 65535) & (T >= 1) & (T <= F)
+    end = off + np.where(ok, T * H * W * 3, 0)
+    rows(ok & ((off < 0) | (end > frames.numel())), f"clip outside the {frames.numel()}-byte frame buffer")
+    tr = mode == 0
+    rows(tr & ((h < 1) | (w < 1)), "crop box h or w < 1")
+    rows(tr & ((i < 0) | (j < 0) | (i + h > H) | (j + w > W)), "crop box outside its frame")
+    ev = (mode == 1) & ok
+    if ev.any():
+        # Source pixels one output index can weigh along an axis (bounded; see egovlp_video_transform_max_taps).
+        shrt, lng = np.minimum(H, W), np.maximum(H, W)
+        nlong = center_crop * lng // shrt
+        d1 = [np.where(W <= H, nlong, center_crop), np.where(W <= H, center_crop, nlong)]
+        sup2 = max(center_crop / R, 1.0)
+        taps = 0
+        for src, dst in zip((H, W), d1):
+            sc1 = src / np.maximum(dst, 1)
+            taps = np.maximum(taps, 2 * sc1 * sup2 + 2 * np.maximum(sc1, 1.0) + 2)
+        rows(ev & (taps > lib().egovlp_video_transform_max_taps()),
+             "source too large for the eval resize (short side above ~7 x center_crop)")
+    if not 1 <= R <= lib().egovlp_video_transform_max_res() or center_crop < 1:
+        bad.append(f"R = {R} outside [1, {lib().egovlp_video_transform_max_res()}] or center_crop = {center_crop} < 1")
+    if bad:
+        raise EgovlpError("video_transform: " + "; ".join(bad))
+    desc_dev = torch.from_numpy(np.ascontiguousarray(d)).to(frames.device, non_blocking=True)
+    out = torch.empty(B, F, 3, R, R, dtype=F32, device=frames.device)
+    m = (C.c_float * 3)(*mean)
+    s = (C.c_float * 3)(*std)
+    call("egovlp_video_transform", _ptr(frames), C.c_longlong(frames.numel()), _ptr(desc_dev), B, F, R, center_crop,
+         m, s, _ptr(out), _stream())
+    return out
+
+
 def video_pos_table(cls_token, pos_embed, temporal_embed, conv_bias, table, T, N, D):
     call("egovlp_video_pos_table", _ptr(cls_token), _ptr(pos_embed), _ptr(temporal_embed), _ptr(conv_bias),
          _ptr(table), T, N, D, _stream())

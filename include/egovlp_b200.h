@@ -126,6 +126,24 @@ int egovlp_patch_im2col(const float* video, void* patches_bf16, int B, int T, in
  * v = (p/255 - mean[c]) / std[c]; host_mean3 / host_std3 are HOST arrays of 3 floats. */
 int egovlp_patch_im2col_u8(const uint8_t* video, void* patches_bf16, int B, int T, int C, int H, int W, int P,
                            const float* host_mean3, const float* host_std3, void* stream);
+/* Dataset video transforms from decoded uint8 frames (replaces, per clip, the reader's `.float() / 255`
+ * (base/base_dataset.py:220-243 and the EgoClip / EPIC / Charades readers), the `init_video_transform_dict` transform
+ * (data_loader/transforms.py:34-61) and the zero-padded `final` copy (base/base_dataset.py:117-140)).
+ *   frames: packed uint8, clip b channels-last [T_b, H_b, W_b, 3] at byte offset desc[b][0]; frames_bytes its size.
+ *   desc: int64 [B, 10] rows (offset, T, H, W, mode, i, j, h, w, flip); mode 0 = train: bilinear resize (no antialias) of
+ *         the crop box rows [i, i + h) x cols [j, j + w) to R x R, then flip != 0 reverses the output columns;
+ *         mode 1 = eval: Resize(center_crop) (short side), CenterCrop(center_crop), Resize(R), both antialiased;
+ *         (i, j, h, w, flip) unused.  T <= F, H, W <= 65535.
+ *   out: fp32 [B, F, 3, R, R] = (resampled p / 255 - mean[c]) / std[c]; frames t >= T are 0.0.  R <=
+ *        egovlp_video_transform_max_res(); the eval weights of one output index may span at most
+ *        egovlp_video_transform_max_taps() source pixels per axis (short side up to ~7 x center_crop at 256 -> 224).
+ *   host_mean / host_std: HOST arrays of 3 floats.
+ * The descriptor table is not checked on the host here (it is device memory): the caller validates it.  A row that
+ * would read outside `frames` is not read; its outputs become NaN. */
+int egovlp_video_transform_max_taps(void);
+int egovlp_video_transform_max_res(void);
+int egovlp_video_transform(const uint8_t* frames, long long frames_bytes, const long long* desc, int B, int F, int R,
+                           int center_crop, const float* host_mean, const float* host_std, float* out, void* stream);
 int egovlp_video_pos_table(const float* cls_token, const float* pos_embed, const float* temporal_embed,
                            const float* conv_bias, float* table, int T, int N, int D, void* stream);
 int egovlp_video_embed_bwd(const float* dx, float* tmp_SD, float* dcls, float* dpos, float* dtemporal, float* dbias,
