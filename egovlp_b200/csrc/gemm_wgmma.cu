@@ -51,7 +51,8 @@ struct EpiParams {
   bf16* out2;
   long long ldr, ldaux, ldo, ldo2;
   int out_mode;  // 0 bf16 store, 1 fp32 store, 2 fp32 atomic add
-  int act;       // 0 none, 1 gelu(erf), 2 multiply by gelu'(aux), 3 gelu(erf) with out2 = gelu', 4 multiply by aux
+  int act;       // 0 none, 1 gelu(erf), 2 multiply by gelu'(aux), 3 gelu(erf) with out2 = gelu', 4 multiply by aux,
+                 // 5 multiply by gelu'(aux) with out2 = gelu(aux)
   float alpha;
   float col_scale;
   int col_scale_ncols;
@@ -186,15 +187,20 @@ __device__ __forceinline__ void gelu2(const GeluConsts& gc, float& x0, float& x1
   f32x2 u, e;
   up2(mul2(x, gelu_phi2(gc, x0, x1, x, u, e)), x0, x1);
 }
-// GELU(x) and GELU'(x) from ONE evaluation of Phi (the fc1 epilogue stores the derivative for the backward instead of
-// the pre-activation: the dgrad-fc2 epilogue then only multiplies, act = 4); both returned packed as bf16x2
-__device__ __forceinline__ void gelu_and_grad2(const GeluConsts& gc, float x0, float x1, uint32_t& g_bf, uint32_t& d_bf) {
+// GELU(x) and GELU'(x) of two elements from ONE evaluation of Phi, in fp32
+__device__ __forceinline__ void gelu_pair2(const GeluConsts& gc, float x0, float x1, float& g0, float& g1, float& d0,
+                                           float& d1) {
   const f32x2 x = pk2(x0, x1);
   f32x2 u, e;
   const f32x2 phi = gelu_phi2(gc, x0, x1, x, u, e);
-  float g0, g1, d0, d1;
   up2(mul2(x, phi), g0, g1);
   up2(fma2(u, e, phi), d0, d1);
+}
+// the same, packed as bf16x2 (the fc1 epilogue stores the derivative for the backward instead of the pre-activation: the
+// dgrad-fc2 epilogue then only multiplies, act = 4)
+__device__ __forceinline__ void gelu_and_grad2(const GeluConsts& gc, float x0, float x1, uint32_t& g_bf, uint32_t& d_bf) {
+  float g0, g1, d0, d1;
+  gelu_pair2(gc, x0, x1, g0, g1, d0, d1);
   g_bf = pack_bf16x2(g0, g1);
   d_bf = pack_bf16x2(d0, d1);
 }
@@ -220,6 +226,9 @@ enum EpiMode {
   EPI_MUL_AUX = 3,   // x bf16 aux -> bf16                                               (Mlp.fc2 input gradient)
   EPI_RES_F32 = 4,   // bias + fp32 residual -> fp32                                     (proj / fc2 forward)
   EPI_ACT1 = 5,      // bias -> GELU -> bf16                                             (Mlp.fc1, inference)
+  // the low-memory training pair: fc1 saves the bf16 pre-activation z, the fc2 input-gradient GEMM rebuilds GELU(z)
+  EPI_ACT1_Z = 6,    // bias -> GELU -> bf16, pre-activation -> bf16 out2                (Mlp.fc1 forward)
+  EPI_GELU_AUX = 7,  // x GELU'(bf16 aux) -> bf16, GELU(aux) -> bf16 out2                (Mlp.fc2 input gradient)
 };
 
 template <int BLOCK_N, bool A_MN, bool B_MN, bool TWO, int MODE>
@@ -236,11 +245,14 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
   const int num_workers = TWO ? (int)(gridDim.x >> 1) : (int)gridDim.x;
   constexpr int STAGES = C::STAGES;
   // TMA-staged epilogue (the specialised forms): subtile width, subtiles per tile, which forms read an input subtile
-  // (the residual or aux, transformed in place) and which write two outputs (GELU and GELU', one buffer each)
+  // (the residual or aux, transformed in place) and which write two outputs.  Without an input the two outputs fill both
+  // buffers of the warpgroup; EPI_GELU_AUX has both, and stores its second output from the input's buffer once the
+  // first output's store has read it, so that the other buffer stays free for the next aux subtile.
   constexpr bool STAGED = MODE != EPI_GENERIC;
   constexpr bool OUT_F32 = MODE == EPI_RES_F32;
-  constexpr bool HAS_IN = MODE == EPI_RES_F32 || MODE == EPI_MUL_AUX;
-  constexpr bool TWO_OUT = MODE == EPI_ACT3;
+  constexpr bool HAS_IN = MODE == EPI_RES_F32 || MODE == EPI_MUL_AUX || MODE == EPI_GELU_AUX;
+  constexpr bool TWO_OUT = MODE == EPI_ACT3 || MODE == EPI_ACT1_Z || MODE == EPI_GELU_AUX;
+  constexpr bool BOTH_BUFS = TWO_OUT && !HAS_IN;
   constexpr int SUB_COLS = OUT_F32 ? 32 : 64;
   constexpr int NSUB = BLOCK_N / SUB_COLS;
   extern __shared__ uint8_t smem_raw[];
@@ -482,9 +494,10 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
         for (int s = 0; s < NSUB; ++s, ++it) {
           const uint32_t b = it % EPI_BUFS, ph = (it / EPI_BUFS) & 1;
           // two outputs fill both buffers: the previous subtile's stores must have read them (the leader waited)
-          if (TWO_OUT) named_bar_sync(1 + mw, 128);
-          const uint32_t buf = sEpi + (mw * EPI_BUFS + (TWO_OUT ? 0u : b)) * EPI_SUB_BYTES;
+          if (BOTH_BUFS) named_bar_sync(1 + mw, 128);
+          const uint32_t buf = sEpi + (mw * EPI_BUFS + (BOTH_BUFS ? 0u : b)) * EPI_SUB_BYTES;
           if (HAS_IN) mbar_wait_nocall(epi_full + 8 * (mw * EPI_BUFS + b), ph);
+          uint32_t second[SUB_COLS / 4];      // EPI_GELU_AUX: GELU(aux), held until the buffer is free for it
 #pragma unroll
           for (int jj = 0; jj < SUB_COLS / 8; ++jj) {
             const int j = s * (SUB_COLS / 8) + jj;        // 8-column group of the tile: constant after unrolling
@@ -501,11 +514,26 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
               if (MODE == EPI_BF16 && n0 + 8 * j + c2 < ep.col_scale_ncols) {
                 v0 = __fmul_rn(v0, ep.col_scale); v1 = __fmul_rn(v1, ep.col_scale);
               }
-              if (MODE == EPI_ACT3) {           // out = GELU(v), out2 = GELU'(v)
+              if (BOTH_BUFS) {                  // ACT3: out = GELU(v), out2 = GELU'(v);  ACT1_Z: out = GELU(v), out2 = v
                 uint32_t g, d;
-                gelu_and_grad2(gc, v0, v1, g, d);
+                if (MODE == EPI_ACT3) {
+                  gelu_and_grad2(gc, v0, v1, g, d);
+                } else {
+                  d = pack_bf16x2(v0, v1);
+                  gelu2(gc, v0, v1);
+                  g = pack_bf16x2(v0, v1);
+                }
                 asm volatile("st.shared.u32 [%0], %1;" ::"r"(buf + off), "r"(g) : "memory");
                 asm volatile("st.shared.u32 [%0], %1;" ::"r"(buf + EPI_SUB_BYTES + off), "r"(d) : "memory");
+              } else if (MODE == EPI_GELU_AUX) {  // out = v GELU'(z), out2 = GELU(z), z = aux
+                uint32_t a;
+                asm volatile("ld.shared.u32 %0, [%1];" : "=r"(a) : "r"(buf + off) : "memory");
+                const float2 z = unpack_bf16x2(a);
+                float g0, g1, d0, d1;
+                gelu_pair2(gc, z.x, z.y, g0, g1, d0, d1);
+                asm volatile("st.shared.u32 [%0], %1;" ::"r"(buf + off),
+                             "r"(pack_bf16x2(__fmul_rn(v0, d0), __fmul_rn(v1, d1))) : "memory");
+                second[2 * jj + h] = pack_bf16x2(g0, g1);
               } else if (MODE == EPI_RES_F32) {
                 float r0, r1;
                 asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(r0), "=f"(r1) : "r"(buf + off) : "memory");
@@ -527,10 +555,29 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
           named_bar_sync(1 + mw, 128);
           if (leader) {
             tma_store_2d(&tmOut, buf, n0 + s * SUB_COLS, m_row);
-            if (TWO_OUT) tma_store_2d(&tmOut2, buf + EPI_SUB_BYTES, n0 + s * SUB_COLS, m_row);
+            if (BOTH_BUFS) tma_store_2d(&tmOut2, buf + EPI_SUB_BYTES, n0 + s * SUB_COLS, m_row);
             bulk_commit();
             bulk_wait_read<0>();
-            if (HAS_IN) mbar_arrive(epi_empty + 8 * (mw * EPI_BUFS + b));
+            if (HAS_IN && !TWO_OUT) mbar_arrive(epi_empty + 8 * (mw * EPI_BUFS + b));
+          }
+          if constexpr (MODE == EPI_GELU_AUX) {
+            named_bar_sync(1 + mw, 128);      // the first output's store has read the buffer
+#pragma unroll
+            for (int jj = 0; jj < SUB_COLS / 8; ++jj)
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const int r = wq * 16 + (lane >> 2) + 8 * h;
+                asm volatile("st.shared.u32 [%0], %1;" ::"r"(buf + r * 128 + ((jj ^ (r & 7)) << 4) + 4 * (lane & 3)),
+                             "r"(second[2 * jj + h]) : "memory");
+              }
+            fence_proxy_async_smem();
+            named_bar_sync(1 + mw, 128);
+            if (leader) {
+              tma_store_2d(&tmOut2, buf, n0 + s * SUB_COLS, m_row);
+              bulk_commit();
+              bulk_wait_read<0>();
+              mbar_arrive(epi_empty + 8 * (mw * EPI_BUFS + b));
+            }
           }
         }
         if (leader) mbar_arrive(bias_empty);      // after the last subtile's warpgroup sync: the bias row is read
@@ -560,14 +607,20 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
             }
             continue;
           }
-          if (ep.out2 && rv)                 // pre-activation (act 1) or a second copy
+          if (ep.out2 && rv && ep.act != 5)  // pre-activation (act 1) or a second copy
             *reinterpret_cast<uint32_t*>(ep.out2 + (long long)row * ep.ldo2 + col) = pack_bf16x2(v0, v1);
           if (ep.act == 1) gelu2(gc, v0, v1);
           const int grow = rv ? row : M - 1;        // clamped: operand loads of padding rows stay in bounds
-          if (ep.act == 2 || ep.act == 4) {
+          if (ep.act == 2 || ep.act == 4 || ep.act == 5) {
             const float2 a = unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(ep.aux + (long long)grow * ep.ldaux + col)));
             if (ep.act == 2) { v0 *= gelu_grad_fast(a.x); v1 *= gelu_grad_fast(a.y); }
-            else { v0 *= a.x; v1 *= a.y; }
+            else if (ep.act == 4) { v0 *= a.x; v1 *= a.y; }
+            else {                           // out = v GELU'(aux), out2 = GELU(aux)
+              float g0, g1, d0, d1;
+              gelu_pair2(gc, a.x, a.y, g0, g1, d0, d1);
+              v0 = __fmul_rn(v0, d0); v1 = __fmul_rn(v1, d1);
+              if (rv) *reinterpret_cast<uint32_t*>(ep.out2 + (long long)row * ep.ldo2 + col) = pack_bf16x2(g0, g1);
+            }
           }
           if (ep.residual) {
             const int rrow = ep.res_row_mod ? grow % ep.res_row_mod : grow;
@@ -620,8 +673,10 @@ int launch(const void* A, long long lda, const void* B, long long ldb, int M, in
     if (!rc) rc = make_tmap_2d_f32(&tmIn, ep.residual, M, N, ep.ldr, EPI_ROWS, 32);
   } else if (STAGED) {
     rc = make_tmap_2d_bf16(&tmOut, ep.out, M, N, ep.ldo, EPI_ROWS, 64);
-    if (!rc && MODE == EPI_ACT3) rc = make_tmap_2d_bf16(&tmOut2, ep.out2, M, N, ep.ldo2, EPI_ROWS, 64);
-    if (!rc && MODE == EPI_MUL_AUX) rc = make_tmap_2d_bf16(&tmIn, ep.aux, M, N, ep.ldaux, EPI_ROWS, 64);
+    if (!rc && (MODE == EPI_ACT3 || MODE == EPI_ACT1_Z || MODE == EPI_GELU_AUX))
+      rc = make_tmap_2d_bf16(&tmOut2, ep.out2, M, N, ep.ldo2, EPI_ROWS, 64);
+    if (!rc && (MODE == EPI_MUL_AUX || MODE == EPI_GELU_AUX))
+      rc = make_tmap_2d_bf16(&tmIn, ep.aux, M, N, ep.ldaux, EPI_ROWS, 64);
   }
   if (rc) return rc;
   constexpr int SMEM_BYTES = STAGED ? C::SMEM_BYTES_STAGED : C::SMEM_BYTES;
@@ -705,6 +760,11 @@ inline int epi_mode(const EpiParams& ep) {
       tma_ok(ep.residual, ep.ldr * 4))
     return EPI_RES_F32;
   if (ep.act == 1 && ep.out_mode == 0 && !ep.residual && !ep.out2 && no_scale && out16) return EPI_ACT1;
+  if (ep.act == 1 && ep.out_mode == 0 && !ep.residual && ep.out2 && no_scale && out16 && tma_ok(ep.out2, ep.ldo2 * 2))
+    return EPI_ACT1_Z;
+  if (ep.act == 5 && ep.out_mode == 0 && !ep.residual && no_scale && out16 && tma_ok(ep.out2, ep.ldo2 * 2) &&
+      tma_ok(ep.aux, ep.ldaux * 2))
+    return EPI_GELU_AUX;
   return EPI_GENERIC;
 }
 
@@ -725,6 +785,8 @@ int dispatch_mode(int a_mn, int b_mn, const void* A, long long lda, const void* 
       case EPI_MUL_AUX: return dispatch_major<BLOCK_N, TWO, EPI_MUL_AUX>(a_mn, b_mn, A, lda, B, ldb, M, N, K, splits, ep, stream);
       case EPI_RES_F32: return dispatch_major<BLOCK_N, TWO, EPI_RES_F32>(a_mn, b_mn, A, lda, B, ldb, M, N, K, splits, ep, stream);
       case EPI_ACT1: return dispatch_major<BLOCK_N, TWO, EPI_ACT1>(a_mn, b_mn, A, lda, B, ldb, M, N, K, splits, ep, stream);
+      case EPI_ACT1_Z: return dispatch_major<BLOCK_N, TWO, EPI_ACT1_Z>(a_mn, b_mn, A, lda, B, ldb, M, N, K, splits, ep, stream);
+      case EPI_GELU_AUX: return dispatch_major<BLOCK_N, TWO, EPI_GELU_AUX>(a_mn, b_mn, A, lda, B, ldb, M, N, K, splits, ep, stream);
       default: break;
     }
   }
@@ -746,9 +808,10 @@ extern "C" int egovlp_gemm_bf16(const void* A, int a_mn_major, long long lda, co
   EGOVLP_CHECK_ARG(lda % 8 == 0 && ldb % 8 == 0, "gemm: leading dimensions must be multiples of 8 (16B TMA strides)");
   EGOVLP_CHECK_ARG((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(B) & 15) == 0,
                    "gemm: operands must be 16B aligned");
-  EGOVLP_CHECK_ARG(e->out_mode >= 0 && e->out_mode <= 2 && e->act >= 0 && e->act <= 4, "gemm: bad epilogue mode");
+  EGOVLP_CHECK_ARG(e->out_mode >= 0 && e->out_mode <= 2 && e->act >= 0 && e->act <= 5, "gemm: bad epilogue mode");
   EGOVLP_CHECK_ARG(split_k <= 1 || e->out_mode == 2, "gemm: split_k > 1 needs out_mode=2 (fp32 atomic accumulate)");
-  EGOVLP_CHECK_ARG((e->act != 2 && e->act != 4) || e->aux, "gemm: act=2/4 needs aux");
+  EGOVLP_CHECK_ARG((e->act != 2 && e->act != 4 && e->act != 5) || e->aux, "gemm: act=2/4/5 needs aux");
+  EGOVLP_CHECK_ARG(e->act != 5 || e->out2, "gemm: act=5 needs out2");
   EGOVLP_CHECK_ARG(e->ldo % 8 == 0, "gemm: ldo must be a multiple of 8");
   EpiParams ep;
   ep.bias = e->bias; ep.residual = e->residual; ep.aux = reinterpret_cast<const bf16*>(e->aux);

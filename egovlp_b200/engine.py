@@ -350,17 +350,37 @@ class PatchEmbedFn(torch.autograd.Function):
         return None, dcls, dpos, dtemp, dw.reshape(D, 3, P, P), dbias, None, None
 
 
+def _ln16(inp, w, b, eps):
+    """-> (bf16 LayerNorm(inp), mean, rstd) of an fp32 [M, D] input (deterministic: a rebuild is bit-identical)."""
+    M, D = inp.shape
+    y = _empty((M, D), BF16, inp)
+    mean, rstd = _empty((M,), F32, inp), _empty((M,), F32, inp)
+    ops.layernorm_fwd(inp, w.detach(), b.detach(), eps, y16=y, mean=mean, rstd=rstd)
+    return y, mean, rstd
+
+
+def _proj_residual(a, pw, pb, resid, cache):
+    """fp32 resid + proj(a): the attention output projection on the bias + fp32 residual GEMM form."""
+    out = _empty(resid.shape, F32, a)
+    ops.gemm(a, cache.get(pw), out, bias=pb.detach(), residual=resid)
+    return out
+
+
 class SpaceTimeBlockFn(torch.autograd.Function):
     """SpaceTimeBlock.forward (model/video_transformer.py:163-177) incl. both VarAttention calls and the Mlp.
 
     params: norm1.{w,b}, attn.qkv.{w,b}, attn.proj.{w,b}, timeattn.qkv.{w,b}, timeattn.proj.{w,b},
             norm2.{w,b}, mlp.fc1.{w,b}, mlp.fc2.{w,b}, norm3.{w,b}      (18 tensors, reference order)
+    dims: (B, T, N, H, grad_mode, low_memory).  low_memory = selective activation recompute for training: the forward
+    saves x, qkv, the attention outputs, the softmax and LayerNorm statistics and the bf16 fc1 pre-activation z (21,624
+    instead of 38,520 bytes per token at D = 768); the backward rebuilds the residuals tr / sr and the LayerNorm outputs
+    from them with the forward's own kernels (bit-identical), and GELU(z) / GELU'(z) inside the fc2 input-gradient GEMM.
     """
 
     @staticmethod
     def forward(ctx, x, dims, eps, cache, *p):
         (n1w, n1b, sqw, sqb, spw, spb, tqw, tqb, tpw, tpb, n2w, n2b, f1w, f1b, f2w, f2b, n3w, n3b) = p
-        B, T, N, H, grad_mode = dims
+        B, T, N, H, grad_mode, low_memory = dims
         D = H * 64
         S = 1 + T * N
         M = B * S
@@ -370,35 +390,51 @@ class SpaceTimeBlockFn(torch.autograd.Function):
         # needs_input_grad reflects requires_grad of the parameters even under torch.no_grad()
         train = grad_mode and any(ctx.needs_input_grad)
 
-        def ln(inp, w, b):
-            y = _empty((M, D), BF16, inp)
-            mean, rstd = _empty((M,), F32, inp), _empty((M,), F32, inp)
-            ops.layernorm_fwd(inp, w.detach(), b.detach(), eps, y16=y, mean=mean, rstd=rstd)
-            return y, mean, rstd
-
         def attention(inp16, qw, qb, pw, pb, mode, resid):
             qkv = _empty((M, 3 * D), BF16, inp16)
             ops.gemm(inp16, cache.get(qw), qkv, bias=qb.detach(), col_scale=Q_SCALE, col_scale_ncols=D)
             a, lse = ops.divided_attn_fwd(qkv, B, T, N, H, mode)
-            out = _empty((M, D), F32, inp16)
-            ops.gemm(a, cache.get(pw), out, bias=pb.detach(), residual=resid)
-            return qkv, a, lse, out
+            return qkv, a, lse, _proj_residual(a, pw, pb, resid, cache)
 
-        n3, mean3, rstd3 = ln(x2, n3w, n3b)
+        n3, mean3, rstd3 = _ln16(x2, n3w, n3b, eps)
         qkv_t, a_t, lse_t, tr = attention(n3, tqw, tqb, tpw, tpb, 0, x2)          # time_residual = x + time_output
-        n1, mean1, rstd1 = ln(tr, n1w, n1b)
+        n1, mean1, rstd1 = _ln16(tr, n1w, n1b, eps)
         qkv_s, a_s, lse_s, sr = attention(n1, sqw, sqb, spw, spb, 1, x2)          # space_residual = x + space_output
-        n2, mean2, rstd2 = ln(sr, n2w, n2b)
+        n2, mean2, rstd2 = _ln16(sr, n2w, n2b, eps)
         h = _empty((M, HID), BF16, x2)
-        u = _empty((M, HID), BF16, x2) if train else None          # GELU'(pre-activation), consumed by the backward
-        ops.gemm(n2, cache.get(f1w), h, bias=f1b.detach(), act=_ACT_FWD if train else 1, out2=u)   # u = GELU'(fc1 output)
+        # training: u = GELU'(fc1 output) for the backward, or in the low-memory mode z = the fc1 output itself (act 1
+        # with out2: h is bit-identical to act 3's)
+        u = _empty((M, HID), BF16, x2) if train else None
+        act = (1 if low_memory else _ACT_FWD) if train else 1
+        ops.gemm(n2, cache.get(f1w), h, bias=f1b.detach(), act=act, out2=u)
         y = _empty((M, D), F32, x2)
         ops.gemm(h, cache.get(f2w), y, bias=f2b.detach(), residual=sr)
         if train:
-            ctx.dims, ctx.cache = (B, T, N, H, HID), cache
-            ctx.save_for_backward(x2, n3, mean3, rstd3, qkv_t, a_t, lse_t, tr, n1, mean1, rstd1, qkv_s, a_s, lse_s, sr,
-                                  n2, mean2, rstd2, u, h, *p)
+            ctx.dims, ctx.cache, ctx.eps = (B, T, N, H, HID), cache, eps
+            if low_memory:          # the None slots are rebuilt by the backward (see `rebuild`)
+                ctx.save_for_backward(x2, None, mean3, rstd3, qkv_t, a_t, lse_t, None, None, mean1, rstd1, qkv_s, a_s,
+                                      lse_s, None, None, mean2, rstd2, u, None, *p)
+            else:
+                ctx.save_for_backward(x2, n3, mean3, rstd3, qkv_t, a_t, lse_t, tr, n1, mean1, rstd1, qkv_s, a_s, lse_s,
+                                      sr, n2, mean2, rstd2, u, h, *p)
         return y.view(B, S, D)
+
+    @staticmethod
+    def rebuild(which, sv, eps, cache):
+        """Rebuild what the low-memory forward did not save, from its saved tensors `sv` (ctx.saved_tensors):
+        'sr' -> (space_residual, bf16 norm2(sr)), 'tr' -> (time_residual, bf16 norm1(tr)), 'n3' -> bf16 norm3(x).
+        The proj GEMM and the LayerNorm forward are deterministic, so the results equal the forward's bit for bit."""
+        x2, a_t, a_s, p = sv[0], sv[5], sv[12], sv[20:]
+        (n1w, n1b, sqw, sqb, spw, spb, tqw, tqb, tpw, tpb, n2w, n2b, f1w, f1b, f2w, f2b, n3w, n3b) = p
+        if which == "sr":
+            r = _proj_residual(a_s, spw, spb, x2, cache)
+            return r, _ln16(r, n2w, n2b, eps)[0]
+        if which == "tr":
+            r = _proj_residual(a_t, tpw, tpb, x2, cache)
+            return r, _ln16(r, n1w, n1b, eps)[0]
+        if which == "n3":
+            return _ln16(x2, n3w, n3b, eps)[0]
+        raise ValueError(which)
 
     @staticmethod
     def backward(ctx, dy):
@@ -423,12 +459,22 @@ class SpaceTimeBlockFn(torch.autograd.Function):
          h) = sv[:20]
         (n1w, n1b, sqw, sqb, spw, spb, tqw, tqb, tpw, tpb, n2w, n2b, f1w, f1b, f2w, f2b, n3w, n3b) = sv[20:]
         dy16, g_f2b = _byproducts_of(dy)                     # fc2 bias gradient = colsum(dy)
+        low_memory = h is None         # rebuild sr / n2, tr / n1 and n3 as they are consumed; free each after its last use
+        if low_memory:
+            sr, n2 = SpaceTimeBlockFn.rebuild("sr", sv, ctx.eps, cache)
 
         # ---- MLP:  y = sr + fc2(gelu(fc1(LN2(sr))))
-        g_f2w = wgrad(dy16, h, D, HID)
-        du = _empty((M, HID), BF16, dy)
-        ops.gemm(dy16, cache.get(f2w), du, b_mn=True, aux=u, act=_ACT_BWD)                # (dy W2) * gelu'
+        if low_memory:             # u = z: du = (dy W2) * gelu'(z), and the same pass writes h = gelu(z) for the wgrad
+            du, h = _empty((M, HID), BF16, dy), _empty((M, HID), BF16, dy)
+            ops.gemm(dy16, cache.get(f2w), du, b_mn=True, aux=u, act=5, out2=h)
+            g_f2w = wgrad(dy16, h, D, HID)
+            del h
+        else:
+            g_f2w = wgrad(dy16, h, D, HID)
+            du = _empty((M, HID), BF16, dy)
+            ops.gemm(dy16, cache.get(f2w), du, b_mn=True, aux=u, act=_ACT_BWD)            # (dy W2) * gelu'
         g_f1w, g_f1b = wgrad_and_bgrad(du, n2, HID, D)       # fc1 bias gradient = colsum(du), summed inside the wgrad GEMM
+        del n2
         dn2 = _empty((M, D), BF16, dy)                       # LayerNorm-input gradients travel as bf16
         ops.gemm(du, cache.get(f1w), dn2, b_mn=True)
         del du
@@ -438,7 +484,7 @@ class SpaceTimeBlockFn(torch.autograd.Function):
         g_spb = _zeros((D,), dy)                             # bias grad of attn.proj = colsum(d space_residual)
         ops.layernorm_bwd(dn2, sr, n2w.detach(), mean2, rstd2, add1=dy, dx16=dsr16, dgamma=g_n2w, dbeta=g_n2b,
                           colsum_dx=g_spb)
-        del dn2
+        del dn2, sr
 
         def attention_bwd(dres16, qkv, a, lse, inp16, qw, pw, mode):
             dres = dres16
@@ -452,14 +498,20 @@ class SpaceTimeBlockFn(torch.autograd.Function):
             return g_qw, g_qb, g_pw, dinp
 
         # ---- space attention:  sr = x + proj(attn(LN1(tr)))
+        if low_memory:
+            tr, n1 = SpaceTimeBlockFn.rebuild("tr", sv, ctx.eps, cache)
         g_sqw, g_sqb, g_spw, dn1 = attention_bwd(dsr16, qkv_s, a_s, lse_s, n1, sqw, spw, 1)
+        del n1
         dtr16 = _empty((M, D), BF16, dy)
         g_n1w, g_n1b = _zeros((D,), dy), _zeros((D,), dy)
         g_tpb = _zeros((D,), dy)                             # bias grad of timeattn.proj = colsum(d time_residual)
         ops.layernorm_bwd(dn1, tr, n1w.detach(), mean1, rstd1, dx16=dtr16, dgamma=g_n1w, dbeta=g_n1b, colsum_dx=g_tpb)
-        del dn1
+        del dn1, tr
         # ---- time attention:  tr = x + proj(timeattn(LN3(x)))
+        if low_memory:
+            n3 = SpaceTimeBlockFn.rebuild("n3", sv, ctx.eps, cache)
         g_tqw, g_tqb, g_tpw, dn3 = attention_bwd(dtr16, qkv_t, a_t, lse_t, n3, tqw, tpw, 0)
+        del n3
         dx, dx16 = _empty((M, D), F32, dy), _empty((M, D), BF16, dy)
         g_n3w, g_n3b = _zeros((D,), dy), _zeros((D,), dy)
         dx_colsum = _zeros((D,), dy)                         # = the fc2 bias gradient of the block below

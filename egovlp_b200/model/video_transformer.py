@@ -87,14 +87,15 @@ class SpaceTimeBlock(nn.Module):
                 self.mlp.fc2.weight, self.mlp.fc2.bias, self.norm3.weight, self.norm3.bias)
 
     def forward(self, x, einops_from_space=None, einops_to_space=None, einops_from_time=None, einops_to_time=None,
-                time_n=None, space_f=None, cache=None):
+                time_n=None, space_f=None, cache=None, low_memory=False):
         """x [B, 1 + space_f*time_n, D] fp32.  The einops pattern arguments of the reference signature are
-        accepted and ignored: the token layout is fixed to the reference's 'b (f n) d'."""
+        accepted and ignored: the token layout is fixed to the reference's 'b (f n) d'.  `low_memory`: selective
+        activation recompute in training (see SpaceTimeTransformer.set_grad_checkpointing)."""
         B = x.shape[0]
         eps = self.norm1.eps
         cache = cache if cache is not None else _default_cache(self)
-        return engine.SpaceTimeBlockFn.apply(x, (B, space_f, time_n, self.num_heads, torch.is_grad_enabled()), eps, cache,
-                                             *self.kernel_params())
+        dims = (B, space_f, time_n, self.num_heads, torch.is_grad_enabled(), bool(low_memory))
+        return engine.SpaceTimeBlockFn.apply(x, dims, eps, cache, *self.kernel_params())
 
 
 def _default_cache(module):
@@ -150,7 +151,16 @@ class SpaceTimeTransformer(nn.Module):
                     nn.init.ones_(m.weight)
         self.einops_from_space, self.einops_to_space = 'b (f n) d', '(b f) n d'
         self.einops_from_time, self.einops_to_time = 'b (f n) d', '(b n) f d'
+        self.grad_checkpointing = False
         object.__setattr__(self, "_bf16_cache", engine.Bf16Cache())
+
+    def set_grad_checkpointing(self, enable=True):
+        """Trade compute for activation memory in training.  This is selective recompute, not timm's re-run of whole
+        blocks: each block keeps its input, the qkv and attention outputs, the softmax / LayerNorm statistics and the bf16
+        fc1 pre-activation (0.56x the activation bytes), and its backward rebuilds the two attention residuals, the three
+        LayerNorm outputs and GELU / GELU' of the pre-activation from them.  The forward, inference and the state_dict
+        are unchanged; the MLP gradients are rounded slightly differently (GELU is taken of the bf16 pre-activation)."""
+        self.grad_checkpointing = bool(enable)
 
     def forward_tokens(self, x, _refresh=True):
         """All tokens after the 12 blocks, [B, S, D] fp32 (before the final norm)."""
@@ -166,7 +176,7 @@ class SpaceTimeTransformer(nn.Module):
                                       pe.proj.bias, cache, getattr(self, "input_norm", None))
         n = (H // pe.patch_size[0]) * (W // pe.patch_size[1])
         for blk in self.blocks:
-            x = blk(x, time_n=n, space_f=F, cache=cache)
+            x = blk(x, time_n=n, space_f=F, cache=cache, low_memory=self.grad_checkpointing)
         return x
 
     def forward_features(self, x, proj=None, _refresh=True):

@@ -43,7 +43,10 @@ int egovlp_abi_version(void);
  *   act 1: v = gelu_erf(v)   act 2: v *= gelu_erf'(aux[m,n]);
  *   act 3: out2[m,n] = bf16(gelu_erf'(v)) (instead of v), then v = gelu_erf(v)   act 4: v *= aux[m,n]
  *          (3 + 4 = the Mlp pair, model/video_transformer.py:46-52: fc1 saves the GELU derivative, the fc2 input-gradient
- *          GEMM only multiplies by it);   v += residual[m,n] (fp32);
+ *          GEMM only multiplies by it);
+ *   act 5: z = aux[m,n]: out2[m,n] = bf16(gelu_erf(z)) (instead of v), then v *= gelu_erf'(z)
+ *          (1 with out2 + 5 = the low-memory Mlp pair: fc1 saves the pre-activation z, and the fc2 input-gradient GEMM
+ *          also rebuilds gelu(z), the fc2 weight gradient's operand);   v += residual[m,n] (fp32);
  *   out_mode 0: out(bf16) = v;  1: out(fp32) = v;  2: atomicAdd(out(fp32), v) (needed for split_k>1)
  * Constraints: N % 32 == 0, lda/ldb/ldo % 8 == 0, 16B-aligned bases.
  * The library chooses the kernel instance itself (tile scheduler, compile-time specialised epilogue for the common
@@ -53,7 +56,7 @@ int egovlp_abi_version(void);
 typedef struct egovlp_gemm_epilogue {
   const float* bias;     /* [N] fp32 or NULL */
   const float* residual; /* [M, ldr] fp32 or NULL */
-  const void* aux;       /* [M, ldaux] bf16, for act == 2 / 4 */
+  const void* aux;       /* [M, ldaux] bf16, for act == 2 / 4 / 5 */
   void* out;             /* [M, ldo] bf16 (out_mode 0) or fp32 (1, 2) */
   void* out2;            /* [M, ldo2] bf16 or NULL */
   long long ldr, ldaux, ldo, ldo2;

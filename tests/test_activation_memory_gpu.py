@@ -1,0 +1,381 @@
+"""Selective activation recompute of the video tower (`SpaceTimeTransformer.set_grad_checkpointing`,
+`video_params["grad_checkpointing"]`):
+  * the two GEMM epilogue forms of the low-memory Mlp pair -- fc1: GELU(v) + the bf16 pre-activation z (act 1 with out2);
+    fc2 input gradient: (dy W2) * GELU'(z) + GELU(z) (act 5) -- bit for bit against the generic epilogue, element-wise
+    against fp64 from the same bf16 operands, and fc1's GELU bit for bit against the default form's (act 3);
+  * the backward's rebuild of tr, sr, n1, n2, n3 equals what the default forward saves, bit for bit;
+  * the saved bytes per token and block: 21,624 instead of 38,520;
+  * the forward (embeddings, loss) is unchanged, and the gradients meet the fp32-oracle tolerances of
+    test_parity_fullsize_gpu.py at the cfg3 shape (B = 8, T = 16) and at the OSCC fine-tuning geometry;
+  * one cfg3 step at B = 64, T = 16, which the default mode cannot fit on an 80 GB card."""
+import gc
+import json
+
+import pytest
+import torch
+
+pytestmark = pytest.mark.gpu
+BF16 = torch.bfloat16
+EMB_TOL, LOSS_TOL = 9e-3, 1e-3
+VIDEO = {"model": "SpaceTimeTransformer", "arch_config": "base_patch16_224", "num_frames": 16, "pretrained": True,
+         "time_init": "zeros"}
+TEXT = {"model": "distilbert-base-uncased", "pretrained": True, "input": "text"}
+SAVED_DEFAULT, SAVED_LOW = 38520, 21624          # bytes per token per block at D = 768, H = 12, HID = 3072
+
+
+@pytest.fixture(scope="module")
+def ops():
+    from egovlp_b200 import ops
+    return ops
+
+
+def mk(shape, seed, scale=1.0, dtype=BF16):
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    return (torch.randn(shape, generator=g, device="cuda") * scale).to(dtype)
+
+
+def rel(a, b):
+    a, b = a.detach().double(), b.detach().double()
+    return ((a - b).norm() / b.norm().clamp_min(1e-30)).item()
+
+
+def cos(a, b):
+    a, b = a.detach().double().flatten(), b.detach().double().flatten()
+    return (a @ b / (a.norm() * b.norm()).clamp_min(1e-300)).item()
+
+
+# ------------------------------------------------------------------------------------------------ epilogue forms
+def run_pair(ops, n2, w1, b1, dy, w2, w2t, z_in):
+    """fc1 forward in both training forms and the fc2 input-gradient form with both B layouts.
+    -> [h (act 1 + out2), z, h (act 3), fc2: du, h(z) with W2 [N, K], du, h(z) with W2^T [K, N]]"""
+    M, HID = n2.shape[0], w1.shape[0]
+    out = [torch.empty(M, HID, device="cuda", dtype=BF16) for _ in range(7)]
+    d = torch.empty(M, HID, device="cuda", dtype=BF16)
+    ops.gemm(n2, w1, out[0], bias=b1, act=1, out2=out[1])
+    ops.gemm(n2, w1, out[2], bias=b1, act=3, out2=d)
+    ops.gemm(dy, w2t, out[3], aux=z_in, act=5, out2=out[4])
+    ops.gemm(dy, w2, out[5], b_mn=True, aux=z_in, act=5, out2=out[6])
+    torch.cuda.synchronize()
+    return out
+
+
+def bf16_ulp(x):
+    e = torch.floor(torch.log2(x.abs().clamp_min(2.0 ** -126)))
+    return torch.exp2(e - 7)
+
+
+def gelu64(x):
+    return x * 0.5 * (1 + torch.erf(x / 2 ** 0.5))
+
+
+def dgelu64(x):
+    return 0.5 * (1 + torch.erf(x / 2 ** 0.5)) + x * torch.exp(-0.5 * x * x) / (2 * torch.pi) ** 0.5
+
+
+def assert_within_ulp(name, got, ref, floor):
+    """|got - ref| <= one bf16 ulp of ref + `floor` (the fp32 accumulation bound and the GELU polynomial's error)."""
+    err = (got.double() - ref).abs()
+    ratio = err / (bf16_ulp(ref) + floor)
+    worst = ratio.max().item()
+    assert worst <= 1.0, (name, worst, err.max().item())
+
+
+def check_vs_fp64(out, n2, w1, b1, dy, w2, z_in, rows):
+    """Element-wise bounds on the rows `rows`.  fp32 accumulation over K terms: <= 2^-20 sum_k |a_k b_k| (a loose form
+    of K 2^-24); the erf polynomial behind GELU / GELU' has |err| <= 1.5e-7, i.e. <= 2e-7 (1 + |x|) on the results."""
+    a, w, bias = n2[rows].double(), w1.double(), b1.double()
+    v = a @ w.t() + bias
+    acc_bound = 2.0 ** -20 * (a.abs() @ w.abs().t() + bias.abs())
+    gelu_bound = 2e-7 * (1 + v.abs())
+    assert_within_ulp("fc1 h", out[0][rows], gelu64(v), 1.13 * acc_bound + gelu_bound)
+    assert_within_ulp("fc1 z", out[1][rows], v, acc_bound)
+    z = z_in[rows].double()
+    g = dy[rows].double() @ w2.double()
+    g_bound = 2.0 ** -20 * (dy[rows].double().abs() @ w2.double().abs())
+    du_ref = g * dgelu64(z)
+    for du, hz in ((out[3], out[4]), (out[5], out[6])):
+        assert_within_ulp("fc2 du", du[rows], du_ref, 1.13 * g_bound + 2e-7 * (1 + z.abs()) * g.abs())
+        assert_within_ulp("fc2 h(z)", hz[rows], gelu64(z), 2e-7 * (1 + z.abs()))
+
+
+@pytest.mark.parametrize("M", [100384, 1001])          # 100,384 = cfg3's 32 clips x 3137 tokens; 1001 is odd
+def test_lowmem_mlp_epilogues_match_generic_and_fp64(ops, monkeypatch, M):
+    """fc1 [M, 768] x [3072, 768]^T and fc2 dgrad [M, 768] x W2 ([768, 3072] stored, i.e. MN-major B, as the backward
+    calls it; plus the same product with W2^T as K-major B), on the specialised forms and on the generic epilogue."""
+    D, HID = 768, 3072
+    n2, w1 = mk((M, D), 1), mk((HID, D), 2, 0.04)
+    b1 = mk((HID,), 3, 0.1, torch.float32)
+    dy, w2 = mk((M, D), 4, 0.5), mk((D, HID), 5, 0.04)
+    w2t = w2.t().contiguous()
+    z_in = mk((M, HID), 6, 1.5)
+    monkeypatch.setenv("EGOVLP_GEMM_GENERIC_EPI", "1")
+    ref = run_pair(ops, n2, w1, b1, dy, w2, w2t, z_in)
+    monkeypatch.setenv("EGOVLP_GEMM_GENERIC_EPI", "0")
+    got = run_pair(ops, n2, w1, b1, dy, w2, w2t, z_in)
+    for i, (r, g) in enumerate(zip(ref, got)):
+        assert torch.equal(r, g), i
+    assert torch.equal(got[0], got[2]), "fc1: GELU of the low-memory form differs from the default (act 3) form's"
+    rows = torch.cat([torch.arange(0, M, 97, device="cuda"), torch.arange(M - 70, M, device="cuda")]).unique()
+    check_vs_fp64(got, n2, w1, b1, dy, w2, z_in, rows)
+
+
+def test_lowmem_mlp_epilogues_on_ragged_shapes_and_pairs(ops, monkeypatch):
+    """Rows past M, 128-column tiles (N = 384) and CTA pairs: still bit for bit the generic epilogue."""
+    for pair in ("0", "1"):
+        monkeypatch.setenv("EGOVLP_GEMM_PAIR", pair)
+        for M, D, HID in ((333, 128, 384), (517, 192, 512)):
+            n2, w1, b1 = mk((M, D), 11), mk((HID, D), 12, 0.1), mk((HID,), 13, 0.1, torch.float32)
+            dy, w2, z_in = mk((M, D), 14), mk((D, HID), 15, 0.1), mk((M, HID), 16)
+            w2t = w2.t().contiguous()
+            monkeypatch.setenv("EGOVLP_GEMM_GENERIC_EPI", "1")
+            ref = run_pair(ops, n2, w1, b1, dy, w2, w2t, z_in)
+            monkeypatch.setenv("EGOVLP_GEMM_GENERIC_EPI", "0")
+            got = run_pair(ops, n2, w1, b1, dy, w2, w2t, z_in)
+            for i, (r, g) in enumerate(zip(ref, got)):
+                assert torch.equal(r, g), (pair, M, i)
+            assert torch.equal(got[0], got[2])
+            check_vs_fp64(got, n2, w1, b1, dy, w2, z_in, torch.arange(M, device="cuda"))
+
+
+def test_lowmem_dgrad_with_misaligned_aux_or_out2_takes_the_generic_epilogue(ops, monkeypatch):
+    """aux / out2 views 8 bytes off 16 (TMA cannot address them): the call takes the generic epilogue and computes the
+    same values as the generic epilogue does by choice, touching only the views."""
+    M, D, HID = 260, 128, 256
+    dy, w2 = mk((M, D), 21), mk((D, HID), 22, 0.1)
+    z_buf = mk((M, HID + 8), 23)
+    z_mis = z_buf[:, 4:4 + HID]
+
+    def run():
+        outs = []
+        for aux_view, off in ((z_mis, 0), (z_buf[:, :HID].contiguous(), 4)):
+            du = torch.empty(M, HID, device="cuda", dtype=BF16)
+            hbuf = torch.zeros(M, HID + 8, device="cuda", dtype=BF16)
+            ops.gemm(dy, w2, du, b_mn=True, aux=aux_view, act=5, out2=hbuf[:, off:off + HID])
+            outs += [du, hbuf]
+        torch.cuda.synchronize()
+        return outs
+
+    monkeypatch.setenv("EGOVLP_GEMM_GENERIC_EPI", "1")
+    ref = run()
+    monkeypatch.setenv("EGOVLP_GEMM_GENERIC_EPI", "0")
+    got = run()
+    for i, (r, g) in enumerate(zip(ref, got)):
+        assert torch.equal(r, g), i
+    g64 = dy.double() @ w2.double()
+    z = z_mis.double()
+    assert rel(got[0], g64 * dgelu64(z)) < 4e-3
+    assert rel(got[1][:, :HID], gelu64(z)) < 4e-3 and torch.all(got[1][:, HID:] == 0)
+    assert torch.all(got[3][:, :4] == 0) and torch.all(got[3][:, 4 + HID:] == 0)
+
+
+# ------------------------------------------------------------------------------------------------ one block
+def _saved_bytes_per_token(fn, M):
+    return sum(t.numel() * t.element_size() for t in fn.saved_tensors[:20] if t is not None) / M
+
+
+def test_block_rebuild_is_bit_identical_and_saved_bytes():
+    """One full-width block (D = 768, 12 heads) at B = 2, T = 16: the rebuilt tr, sr, n1, n2, n3 equal what the default
+    forward saved, bit for bit; the block output is the same; saved bytes per token are 38,520 and 21,624; the two
+    backwards agree to the rounding of the MLP gradient."""
+    from egovlp_b200 import engine
+    from egovlp_b200.model.video_transformer import SpaceTimeBlock
+    torch.manual_seed(0)
+    blk = SpaceTimeBlock(768, 12, qkv_bias=True, norm_layer=lambda d: torch.nn.LayerNorm(d, eps=1e-6),
+                         time_init="rand").cuda()
+    B, T, N = 2, 16, 196
+    M = B * (1 + T * N)
+    x = torch.randn(B, 1 + T * N, 768, device="cuda")
+    probe = torch.randn(B, 1 + T * N, 768, device="cuda")
+    outs, grads = [], []
+    for low in (False, True):
+        blk.zero_grad(set_to_none=True)
+        xi = x.clone().requires_grad_(True)
+        y = blk(xi, time_n=N, space_f=T, low_memory=low)
+        outs.append((y, y.grad_fn))
+        (y * probe).sum().backward(retain_graph=True)
+        grads.append({k: p.grad.clone() for k, p in blk.named_parameters()} | {"x": xi.grad.clone()})
+    (y0, f0), (y1, f1) = outs
+    assert torch.equal(y0, y1)
+    s0, s1 = f0.saved_tensors, f1.saved_tensors
+    assert all(s1[i] is None for i in (1, 7, 8, 14, 15, 19))
+    sr, n2 = engine.SpaceTimeBlockFn.rebuild("sr", s1, f1.eps, f1.cache)
+    tr, n1 = engine.SpaceTimeBlockFn.rebuild("tr", s1, f1.eps, f1.cache)
+    n3 = engine.SpaceTimeBlockFn.rebuild("n3", s1, f1.eps, f1.cache)
+    for name, got, i in (("n3", n3, 1), ("tr", tr, 7), ("n1", n1, 8), ("sr", sr, 14), ("n2", n2, 15)):
+        assert torch.equal(got, s0[i]), name
+    b0, b1 = _saved_bytes_per_token(f0, M), _saved_bytes_per_token(f1, M)
+    print(f"\n[block B=2 T=16] saved bytes per token: default {b0:.0f}, low-memory {b1:.0f}")
+    assert b0 == SAVED_DEFAULT and b1 == SAVED_LOW
+    worst = min((cos(grads[1][k], grads[0][k]), k) for k in grads[0])
+    print(f"[block B=2 T=16] lowest gradient cosine low-memory vs default: {worst[0]:.7f} ({worst[1]})")
+    assert worst[0] > 0.9995, worst
+
+
+def test_config_key_and_method_switch_the_mode():
+    from egovlp_b200.model.model import FrozenInTime
+    from egovlp_b200.model.video_transformer import SpaceTimeTransformer
+    assert FrozenInTime(dict(VIDEO), TEXT).video_model.grad_checkpointing is False
+    net = FrozenInTime(dict(VIDEO, grad_checkpointing=True), TEXT)
+    assert net.video_model.grad_checkpointing is True
+    tower = SpaceTimeTransformer(img_size=32, patch_size=16, embed_dim=128, depth=2, num_heads=2, num_frames=4,
+                                 num_classes=0).cuda()
+    assert tower.grad_checkpointing is False
+    keys, text = list(tower.state_dict()), str(tower)
+    video = torch.randn(2, 4, 3, 32, 32, device="cuda")
+
+    def block_saves_h():
+        x = tower.forward_tokens(video)
+        return x.grad_fn.saved_tensors[19] is not None
+
+    assert block_saves_h()
+    tower.set_grad_checkpointing()
+    assert tower.grad_checkpointing is True and not block_saves_h()
+    assert list(tower.state_dict()) == keys and str(tower) == text
+    tower.set_grad_checkpointing(False)
+    assert block_saves_h()
+
+
+# ------------------------------------------------------------------------------------------------ whole model
+@pytest.fixture(scope="module")
+def cfg3_runs():
+    """The cfg3 step at B = 8, T = 16 in both modes on one network and inputs, and the fp32 oracle's."""
+    from egovlp_b200 import synthetic as syn
+    from egovlp_b200.model.loss import EgoNCE
+    from egovlp_b200.model.model import FrozenInTime
+    from oracle import reference_port as rp
+    torch.backends.cuda.matmul.allow_tf32 = False
+    torch.backends.cudnn.allow_tf32 = False
+    sd = syn.seeded_state_dict(syn.model_dims(num_frames=16), seed=0)
+    net = FrozenInTime(dict(VIDEO), TEXT)
+    net.load_state_dict(sd, strict=True)
+    net.text_model.config.dropout = net.text_model.config.attention_dropout = 0.0
+    net.cuda()
+    B, T, L = 8, 16, 16
+    data = {"video": syn.synthetic_video(B, T, seed=5).cuda(),
+            "text": {k: v.cuda() for k, v in syn.synthetic_text(B, L, seed=5, ragged=True).items()}}
+    verb, noun = [t.cuda() for t in syn.synthetic_tags(B, seed=5)]
+    runs = {}
+    for low in (False, True):
+        net.video_model.set_grad_checkpointing(low)
+        net.zero_grad(set_to_none=True)
+        t, v = net(data)
+        loss = EgoNCE().fused(t, v, verb, noun)
+        loss.backward()
+        runs[low] = (t.detach().clone(), v.detach().clone(), loss.detach().clone(),
+                     {k: w.grad.clone() for k, w in net.named_parameters() if w.grad is not None})
+    net.video_model.set_grad_checkpointing(False)
+    p = {k: w.cuda().clone().requires_grad_(True) for k, w in sd.items()}
+    tr, vr = rp.frozen_in_time_forward(data, p)
+    lr = rp.egonce_loss(rp.sim_matrix(tr, vr), rp.sim_matrix(verb, verb), rp.sim_matrix(noun, noun))
+    lr.backward()
+    oracle = (tr.detach(), vr.detach(), lr.detach(), {k: q.grad for k, q in p.items() if q.grad is not None})
+    return runs, oracle
+
+
+def test_cfg3_forward_is_unchanged(cfg3_runs):
+    runs, _ = cfg3_runs
+    for a, b in zip(runs[False][:3], runs[True][:3]):
+        assert torch.equal(a, b)
+
+
+def test_cfg3_b8_t16_gradients_vs_fp32_oracle_and_default(cfg3_runs):
+    runs, (tr, vr, lr, g_ref) = cfg3_runs
+    t, v, loss, g = runs[True]
+    g_def = runs[False][3]
+    e_t, e_v, e_l = rel(t, tr), rel(v, vr), abs(loss.item() - lr.item()) / abs(lr.item())
+    rows = [(k, cos(g[k], g_ref[k]), g_ref[k].numel()) for k in g_ref
+            if k in g and g_ref[k].norm().item() >= 1e-12 and not k.endswith("k_lin.bias")]
+    worst_m = min((r for r in rows if r[2] > 4096), key=lambda r: r[1])
+    keys = [k for k in g_ref if k in g]
+    cos_all = cos(torch.cat([g[k].double().flatten() for k in keys]), torch.cat([g_ref[k].double().flatten() for k in keys]))
+    mats = [k for k, _, n in rows if n > 4096]
+    vs_def = min((cos(g[k], g_def[k]), k) for k in mats)
+    worst_def = min((cos(g_def[k], g_ref[k]), k) for k in mats)
+    payload = {"rel_text_emb": e_t, "rel_video_emb": e_v, "rel_loss": e_l, "grad_cos_all": cos_all,
+               "worst_matrix_vs_oracle": worst_m[:2], "default_mode_worst_matrix_vs_oracle": worst_def,
+               "worst_matrix_vs_default": vs_def, "n_tensors": len(rows)}
+    print("\n[cfg3 B=8 T=16, low-memory mode]", json.dumps(payload))
+    assert len(rows) >= 318, len(rows)
+    assert e_t < EMB_TOL and e_v < EMB_TOL and e_l < LOSS_TOL, payload
+    assert cos_all > 0.997 and worst_m[1] > 0.993, payload
+    # no farther from fp32 than the default mode is
+    assert worst_m[1] > worst_def[0] - 1e-3, payload
+    # The two modes round the MLP gradient differently, and that difference grows through 12 blocks like any other
+    # rounding: the two modes then differ by about the sum of their own distances from fp32 (1 - cos adds up).  Measured
+    # on an H100: lowest 0.99894 and 0.99901 in two runs, on video_model.pos_embed (a sum over all clips and frames;
+    # the weight-gradient GEMMs accumulate with fp32 atomics, so the backward varies in its last bits from run to run).
+    assert vs_def[0] > 0.998, payload
+
+
+def test_oscc_step_b4_t16_vs_fp32_oracle():
+    """The OSCC fine-tuning step (4 clips x 16 frames, 2-wide head, cross-entropy) in the low-memory mode."""
+    from egovlp_b200 import synthetic as syn
+    from egovlp_b200.distributed import AllGatherLocalGrad
+    from egovlp_b200.model.loss import CrossEntropy
+    from egovlp_b200.model.model import FrozenInTime
+    from oracle import finetune_port as fp, reference_port as rp
+    torch.backends.cuda.matmul.allow_tf32 = False
+    torch.backends.cudnn.allow_tf32 = False
+    net = FrozenInTime(dict(VIDEO, grad_checkpointing=True), TEXT, projection_dim=2)
+    net.load_state_dict(syn.seeded_state_dict(syn.model_dims(num_frames=16, proj_dim=2), seed=13), strict=True)
+    net.cuda()
+    video = syn.synthetic_video(4, 16, seed=31).cuda()
+    state = torch.tensor([1, 0, 0, 1]).cuda()
+    scores = net({"video": video}, video_only=True)
+    loss = CrossEntropy()(AllGatherLocalGrad.apply(scores), AllGatherLocalGrad.apply(state))
+    loss.backward()
+    p = {k: v.detach().clone().requires_grad_(True) for k, v in net.state_dict().items()
+         if k.startswith(("video_model.", "vid_proj."))}
+    sr = rp.compute_video(video, p)
+    sr.retain_grad()
+    lr = fp.oscc_step_loss([sr], [state])
+    lr.backward()
+    params = dict(net.named_parameters())
+    rows = [(k, cos(params[k].grad, q.grad), q.grad.numel()) for k, q in p.items() if q.grad.norm() > 1e-12]
+    c_all = cos(torch.cat([params[k].grad.double().flatten() for k, _, _ in rows]),
+                torch.cat([p[k].grad.double().flatten() for k, _, _ in rows]))
+    worst_m = min((r for r in rows if r[2] > 4096), key=lambda r: r[1])
+    e_logit = rel(scores, sr)
+    # as the default mode's OSCC test: 2-wide logits pass their bf16 error to the loss at first order, so the loss is held
+    # to |dL| <= ||dL/dz|| ||dz|| with 10 % slack
+    loss_bound = 1.1 * sr.grad.double().norm().item() * (scores.detach().double() - sr.detach().double()).norm().item()
+    print(f"\n[oscc B=4 T=16 low-memory vs fp32 oracle] logits rel-L2 {e_logit:.2e}, |dL| {abs(loss.item() - lr.item()):.2e}"
+          f" (bound {loss_bound:.2e}), whole-gradient cosine {c_all:.5f}, lowest matrix cosine {worst_m[1]:.5f}")
+    assert e_logit < EMB_TOL and abs(loss.item() - lr.item()) <= loss_bound
+    assert c_all > 0.997 and worst_m[1] > 0.993 and len(rows) >= 150
+
+
+def test_cfg3_step_b64_t16_fits():
+    """One cfg3 training step (EgoNCE, fused AdamW) at 64 clips x 16 frames in the low-memory mode."""
+    from egovlp_b200 import synthetic as syn
+    from egovlp_b200.distributed import egoclip_step_loss
+    from egovlp_b200.model.loss import EgoNCE
+    from egovlp_b200.model.model import FrozenInTime
+    from egovlp_b200.optim import AdamW
+    B, T, L = 64, 16, 16
+    tokens = B * (1 + T * 196)
+    # saved activations of 12 blocks + one block backward's transients (~30 KB per token) + weights, gradients, Adam
+    # state and the text tower (~4 GB)
+    need = 12 * SAVED_LOW * tokens + 30e3 * tokens + 4e9
+    gc.collect()
+    torch.cuda.empty_cache()                   # blocks this process's allocator caches count as used by the card
+    free = torch.cuda.mem_get_info()[0]
+    if free < need:
+        pytest.skip(f"needs ~{need / 1e9:.0f} GB free on the card, {free / 1e9:.0f} GB are (the card is shared)")
+    net = FrozenInTime(dict(VIDEO, grad_checkpointing=True), TEXT)
+    net.load_state_dict(syn.seeded_state_dict(syn.model_dims(num_frames=16), seed=0), strict=True)
+    net.cuda()
+    opt = AdamW(net.parameters(), lr=3e-5)
+    txt = syn.synthetic_text(B, L, seed=0)
+    verb, noun = syn.synthetic_tags(B, seed=0)
+    data = {"video": syn.synthetic_video(B, T, seed=0).cuda(), "text": {k: v.cuda() for k, v in txt.items()},
+            "verb_vec": verb.cuda(), "noun_vec": noun.cuda()}
+    torch.cuda.reset_peak_memory_stats()
+    opt.zero_grad(set_to_none=True)
+    loss = egoclip_step_loss(net, EgoNCE(), data)
+    loss.backward()
+    opt.step()
+    torch.cuda.synchronize()
+    peak = torch.cuda.max_memory_allocated()
+    print(f"\n[cfg3 B=64 T=16 low-memory] loss {loss.item():.5f}, peak allocated {peak / 1e9:.1f} GB")
+    assert torch.isfinite(loss).item()
