@@ -222,6 +222,13 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, uint32_t src,
                ::"l"(reinterpret_cast<uint64_t>(m)), "r"(src), "r"(c0), "r"(c1)
                : "memory");
 }
+// TMA reduce smem -> global: adds the box element-wise into the tensor (fp32 add in L2, like red.global.add; rows /
+// columns outside the tensor are clipped), tracked by the issuing thread's bulk groups like a store
+__device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* m, uint32_t src, int c0, int c1) {
+  asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(src), "r"(c0), "r"(c1)
+               : "memory");
+}
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 // at most N of this thread's bulk groups still READ their smem source (the buffers of the others may be rewritten)
 template <int N>

@@ -26,7 +26,8 @@
 // descriptor, everything else takes the generic epilogue (same arithmetic, same order: bit-identical results).  The
 // specialised epilogues move their HBM bytes by TMA: the bias row and the residual / aux subtiles arrive in shared
 // memory while the tile's k-blocks run, and the results leave through 128B-swizzled staging subtiles as TMA stores that
-// drain while the math warpgroups already run the next tile.  The generic epilogue loads and stores from registers.
+// drain while the math warpgroups already run the next tile.  The split-K weight gradients leave the same way: each
+// unit's fp32 partial tile is added into dW by TMA reduce.  The generic epilogue loads and stores from registers.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -229,6 +230,8 @@ enum EpiMode {
   // the low-memory training pair: fc1 saves the bf16 pre-activation z, the fc2 input-gradient GEMM rebuilds GELU(z)
   EPI_ACT1_Z = 6,    // bias -> GELU -> bf16, pre-activation -> bf16 out2                (Mlp.fc1 forward)
   EPI_GELU_AUX = 7,  // x GELU'(bf16 aux) -> bf16, GELU(aux) -> bf16 out2                (Mlp.fc2 input gradient)
+  // the weight gradients (MN-major A and B, split-K): each unit's fp32 partial tile is added into dW by TMA reduce
+  EPI_RED_F32 = 8,   // alpha -> fp32 add into out                                      (every wgrad)
 };
 
 template <int BLOCK_N, bool A_MN, bool B_MN, bool TWO, int MODE>
@@ -249,7 +252,8 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
   // buffers of the warpgroup; EPI_GELU_AUX has both, and stores its second output from the input's buffer once the
   // first output's store has read it, so that the other buffer stays free for the next aux subtile.
   constexpr bool STAGED = MODE != EPI_GENERIC;
-  constexpr bool OUT_F32 = MODE == EPI_RES_F32;
+  constexpr bool RED = MODE == EPI_RED_F32;      // no bias row and no input: warp 1 and the bias barriers stay idle
+  constexpr bool OUT_F32 = MODE == EPI_RES_F32 || RED;
   constexpr bool HAS_IN = MODE == EPI_RES_F32 || MODE == EPI_MUL_AUX || MODE == EPI_GELU_AUX;
   constexpr bool TWO_OUT = MODE == EPI_ACT3 || MODE == EPI_ACT1_Z || MODE == EPI_GELU_AUX;
   constexpr bool BOTH_BUFS = TWO_OUT && !HAS_IN;
@@ -398,7 +402,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
           red_add_v4(ep.colsum_a + col + 4, acc[4], acc[5], acc[6], acc[7]);
         }
       }
-    } else if (STAGED && warp == 1) {
+    } else if (STAGED && !RED && warp == 1) {
       // ===================== epilogue inputs (TMA), while the math warpgroups run the tile's k-blocks =====================
       // Per tile: the bias row once the previous tile's epilogue has consumed it, then the residual / aux subtiles of
       // both warpgroups into their buffer rings as the stores of earlier subtiles free them.  Rows >= M and columns >= N
@@ -489,7 +493,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
         // back to the input warp (or rewritten).  The global writes drain while the next subtile / tile runs.
         const int m_row = m_blk * TILE_M + (int)rank * BLOCK_M + mw * EPI_ROWS, n0 = n_blk * BLOCK_N;
         const int c2 = 2 * (lane & 3);
-        mbar_wait_nocall(bias_full, tc & 1);
+        if (!RED) mbar_wait_nocall(bias_full, tc & 1);
 #pragma unroll
         for (int s = 0; s < NSUB; ++s, ++it) {
           const uint32_t b = it % EPI_BUFS, ph = (it / EPI_BUFS) & 1;
@@ -501,8 +505,9 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
 #pragma unroll
           for (int jj = 0; jj < SUB_COLS / 8; ++jj) {
             const int j = s * (SUB_COLS / 8) + jj;        // 8-column group of the tile: constant after unrolling
-            float2 bq;
-            asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(bq.x), "=f"(bq.y) : "r"(sBias + 4 * (8 * j + c2)));
+            float2 bq = make_float2(0.f, 0.f);
+            if (!RED)
+              asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(bq.x), "=f"(bq.y) : "r"(sBias + 4 * (8 * j + c2)));
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
               const int r = wq * 16 + (lane >> 2) + 8 * h;  // row of the subtile; 16-byte chunks XOR-swizzled by r & 7
@@ -534,6 +539,8 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
                 asm volatile("st.shared.u32 [%0], %1;" ::"r"(buf + off),
                              "r"(pack_bf16x2(__fmul_rn(v0, d0), __fmul_rn(v1, d1))) : "memory");
                 second[2 * jj + h] = pack_bf16x2(g0, g1);
+              } else if (RED) {
+                asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(buf + off), "f"(v0), "f"(v1) : "memory");
               } else if (MODE == EPI_RES_F32) {
                 float r0, r1;
                 asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(r0), "=f"(r1) : "r"(buf + off) : "memory");
@@ -554,7 +561,8 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
           fence_proxy_async_smem();
           named_bar_sync(1 + mw, 128);
           if (leader) {
-            tma_store_2d(&tmOut, buf, n0 + s * SUB_COLS, m_row);
+            if (RED) tma_reduce_add_2d(&tmOut, buf, n0 + s * SUB_COLS, m_row);
+            else tma_store_2d(&tmOut, buf, n0 + s * SUB_COLS, m_row);
             if (BOTH_BUFS) tma_store_2d(&tmOut2, buf + EPI_SUB_BYTES, n0 + s * SUB_COLS, m_row);
             bulk_commit();
             bulk_wait_read<0>();
@@ -580,7 +588,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
             }
           }
         }
-        if (leader) mbar_arrive(bias_empty);      // after the last subtile's warpgroup sync: the bias row is read
+        if (!RED && leader) mbar_arrive(bias_empty);      // after the last subtile's warpgroup sync: the bias row is read
       } else {
       const int row_lo = m_blk * TILE_M + (int)rank * BLOCK_M + mw * 64 + wq * 16 + (lane >> 2);
       const int col_base = n_blk * BLOCK_N + 2 * (lane & 3);
@@ -668,9 +676,9 @@ int launch(const void* A, long long lda, const void* B, long long ldb, int M, in
   // epilogue subtiles of the staged forms: [64 rows, 128 B] boxes over out / out2 / residual / aux
   constexpr bool STAGED = MODE != EPI_GENERIC;
   CUtensorMap tmOut = {}, tmOut2 = {}, tmIn = {};
-  if (MODE == EPI_RES_F32) {
+  if (MODE == EPI_RES_F32 || MODE == EPI_RED_F32) {
     rc = make_tmap_2d_f32(&tmOut, ep.out, M, N, ep.ldo, EPI_ROWS, 32);
-    if (!rc) rc = make_tmap_2d_f32(&tmIn, ep.residual, M, N, ep.ldr, EPI_ROWS, 32);
+    if (!rc && MODE == EPI_RES_F32) rc = make_tmap_2d_f32(&tmIn, ep.residual, M, N, ep.ldr, EPI_ROWS, 32);
   } else if (STAGED) {
     rc = make_tmap_2d_bf16(&tmOut, ep.out, M, N, ep.ldo, EPI_ROWS, 64);
     if (!rc && (MODE == EPI_ACT3 || MODE == EPI_ACT1_Z || MODE == EPI_GELU_AUX))
@@ -765,6 +773,8 @@ inline int epi_mode(const EpiParams& ep) {
   if (ep.act == 5 && ep.out_mode == 0 && !ep.residual && no_scale && out16 && tma_ok(ep.out2, ep.ldo2 * 2) &&
       tma_ok(ep.aux, ep.ldaux * 2))
     return EPI_GELU_AUX;
+  if (ep.act == 0 && ep.out_mode == 2 && !ep.bias && !ep.residual && !ep.out2 && no_scale && tma_ok(ep.out, ep.ldo * 4))
+    return EPI_RED_F32;
   return EPI_GENERIC;
 }
 
@@ -789,6 +799,8 @@ int dispatch_mode(int a_mn, int b_mn, const void* A, long long lda, const void* 
       case EPI_GELU_AUX: return dispatch_major<BLOCK_N, TWO, EPI_GELU_AUX>(a_mn, b_mn, A, lda, B, ldb, M, N, K, splits, ep, stream);
       default: break;
     }
+  } else if (b_mn && epi_mode(ep) == EPI_RED_F32) {      // the weight gradients: split-K partial tiles added by TMA
+    return launch<BLOCK_N, true, true, false, EPI_RED_F32>(A, lda, B, ldb, M, N, K, splits, ep, stream);
   }
   return dispatch_major<BLOCK_N, TWO>(a_mn, b_mn, A, lda, B, ldb, M, N, K, splits, ep, stream);
 }

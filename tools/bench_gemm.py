@@ -1,12 +1,14 @@
 """Per-form timing of the GEMM calls one video block (SpaceTimeBlockFn) makes at the headline step's size.
 
-    python tools/bench_gemm.py [--M 100384] [--iters 20] [--json out.json]
+    python tools/bench_gemm.py [--M 100384] [--iters 20] [--json out.json] [--wgrad-decomp]
 
 cfg3 = 32 clips x (1 + 16 x 196) tokens = 100,384 rows.  Every call of engine.py's forward and input-gradient GEMMs is
 timed with CUDA events, with the same dtypes, epilogue arguments and b_mn flags, plus the weight gradients with
 engine._split_for's split.  A form that reads or writes more than one bf16 output's worth of epilogue bytes is also timed
 with the plain bf16 epilogue on the same A.B: the difference is what its epilogue costs on top.  Each specialised form is
-checked bit for bit against the generic epilogue (EGOVLP_GEMM_GENERIC_EPI=1) at this size.
+checked bit for bit against the generic epilogue (EGOVLP_GEMM_GENERIC_EPI=1) at this size.  The block's six weight
+gradients are summed with their TFLOP/s; --wgrad-decomp also times each of them without the fused bias gradient,
+through the K-major form on transposed copies (the operand path's share) and at the splits around the engine's choice.
 EGOVLP_B200_LIB=<path> runs another build of the library (A/B comparisons)."""
 import argparse
 import json
@@ -51,6 +53,9 @@ def main():
     ap.add_argument("--M", type=int, default=32 * (1 + 16 * 196))
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--json", default=None)
+    ap.add_argument("--wgrad-decomp", action="store_true",
+                    help="also time each weight gradient without the bias gradient, through the K-major form on "
+                         "transposed copies, and at the splits around the engine's choice")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "bench_gemm.py measures on the GPU"
     M, dev = args.M, "cuda"
@@ -118,7 +123,8 @@ def main():
         report["forms"].append(dict(name=name, calls_per_block=n, ms=ms, tflops=flop / ms / 1e9, epilogue_mb=ebytes / 1e6,
                                     plain_bf16_ms=plain_ms, bitwise_equal_generic=same))
     os.environ.pop("EGOVLP_GEMM_GENERIC_EPI", None)
-    # weight gradients (split-K fp32 atomics, generic epilogue), the engine's split rule
+    # weight gradients (MN-major dy and x, split-K fp32 adds into dW), the engine's split rule
+    wgrad_block, decomp = 0.0, []
     for name, n, dy, x, n_out, n_in, colsum in [("fc2 wgrad", 1, dy768, x3072, D, HID, False),
                                                 ("fc1 wgrad (+ bias grad)", 1, dy3072, x768, HID, D, True),
                                                 ("proj wgrad", 2, dy768, x768, D, D, False),
@@ -130,8 +136,22 @@ def main():
                    args.iters)
         flop = 2.0 * M * n_out * n_in
         ms_block += n * ms
+        wgrad_block += n * ms
         rows.append((f"{name} split {split}", n, ms, flop / ms / 1e9, n_out * n_in * 4 / 1e6, None, None))
         report["forms"].append(dict(name=name, split=split, calls_per_block=n, ms=ms, tflops=flop / ms / 1e9))
+        if args.wgrad_decomp:
+            # where the wgrad time goes: without the fused bias gradient; the same product through the K-major form
+            # (transposed copies made here, outside the timed region; the forward / dgrad operand path) at the same
+            # split; and the MN/MN form at the splits around the engine's choice (wave fill, flush count)
+            d = dict(name=name, split=split)
+            mn = lambda s: lambda: ops.gemm(dy, x, dw, a_mn=True, b_mn=True, accumulate=True, split_k=s)  # noqa: E731
+            d["no_colsum_ms"] = timed(mn(split), args.iters)
+            dyt, xt = dy.t().contiguous(), x.t().contiguous()
+            d["kmajor_ms"] = timed(lambda: ops.gemm(dyt, xt, dw, accumulate=True, split_k=split), args.iters)
+            del dyt, xt
+            d["splits_ms"] = {s: timed(mn(s), args.iters) for s in range(max(1, split - 3), split + 4)}
+            decomp.append(d)
+    report["wgrad_decomposition"] = decomp
 
     print(f"GPU: {report['gpu']}   (name, power limit, SM clock, max SM clock)")
     print(f"M = {M}, library: {report['lib']}")
@@ -143,7 +163,15 @@ def main():
         print(f"{name:40s} {n:5d} {ms:8.3f} {tf:8.1f} {mb:8.1f} {pl} {sc}  {eq}")
     print(f"per block: GEMMs {ms_block:.3f} ms, epilogue surcharge {surcharge_block:.3f} ms; "
           f"x 12 blocks: {12 * ms_block:.1f} ms, surcharge {12 * surcharge_block:.1f} ms")
-    report.update(block_ms=ms_block, block_surcharge_ms=surcharge_block, mismatches=mismatches)
+    # the block's six weight gradients (qkv and proj twice, fc1, fc2) do the FLOPs of its forward GEMMs
+    wgrad_flop = 2.0 * M * (2 * 3 * D * D + 2 * D * D + D * HID + HID * D)
+    print(f"per block: weight gradients {wgrad_block:.3f} ms = {wgrad_flop / wgrad_block / 1e9:.1f} TFLOP/s")
+    for d in decomp:
+        sp = "  ".join(f"{s}:{t:.3f}" for s, t in d["splits_ms"].items())
+        print(f"  {d['name']:28s} split {d['split']}: no colsum {d['no_colsum_ms']:.3f} ms, K-major operands "
+              f"{d['kmajor_ms']:.3f} ms, by split  {sp}")
+    report.update(block_ms=ms_block, block_surcharge_ms=surcharge_block, mismatches=mismatches,
+                  wgrad_block_ms=wgrad_block, wgrad_block_tflops=wgrad_flop / wgrad_block / 1e9)
     if args.json:
         with open(args.json, "w") as f:
             json.dump(report, f, indent=1)
