@@ -92,6 +92,14 @@ int make_tmap_2d_f32(CUtensorMap* out, const void* base, uint64_t rows, uint64_t
   return make_tmap_nd(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, base, 2, dims, strides, box, true);
 }
 
+int make_tmap_2d_u8(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows,
+                    uint32_t box_cols) {
+  const uint64_t dims[2] = {cols, rows};
+  const uint64_t strides[2] = {1, ld};
+  const uint32_t box[2] = {box_cols, box_rows};
+  return make_tmap_nd(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, base, 2, dims, strides, box, true);
+}
+
 }  // namespace egovlp
 
 extern "C" const char* egovlp_last_error(void) { return egovlp::g_err; }

@@ -59,6 +59,22 @@ __device__ __forceinline__ float warp_max(float v) {
   return v;
 }
 
+// fp8 e4m3 (e4m3fn: no infinities, largest finite 448) operands with one fp32 scale per row: scale = amax / 448 (1 for
+// a row without a nonzero value) and the stored values x * (448 / amax), converted round-to-nearest-even with
+// saturation to +-448 (NaN stays NaN).  Both divisions are correctly rounded whatever the compile flags.
+constexpr float E4M3_MAX = 448.f;
+__device__ __forceinline__ void e4m3_row_scale(float amax, float& scale, float& inv) {
+  if (amax > 0.f) { scale = __fdiv_rn(amax, E4M3_MAX); inv = __fdiv_rn(E4M3_MAX, amax); }
+  else { scale = 1.f; inv = 1.f; }
+}
+// four consecutive values -> four e4m3 bytes, a first (lowest address)
+__device__ __forceinline__ uint32_t pack_e4m3x4(float a, float b, float c, float d) {
+  uint16_t lo, hi;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(lo) : "f"(b), "f"(a));     // first source -> upper byte
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(hi) : "f"(d), "f"(c));
+  return (uint32_t)lo | ((uint32_t)hi << 16);
+}
+
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&v);
@@ -299,6 +315,9 @@ int make_tmap_2d_bf16(CUtensorMap* out, const void* base, uint64_t rows, uint64_
 // the same for fp32 (box_cols * 4 bytes must be 128)
 int make_tmap_2d_f32(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows,
                      uint32_t box_cols);
+// the same for bytes (e4m3; box_cols must be 128)
+int make_tmap_2d_u8(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows,
+                    uint32_t box_cols);
 // Generic N-d (<=5) bf16 map: dims/strides innermost first, strides in elements (stride[0] must be 1).
 int make_tmap_nd_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides,
                       const uint32_t* box, bool swizzle128);

@@ -28,6 +28,8 @@
 // memory while the tile's k-blocks run, and the results leave through 128B-swizzled staging subtiles as TMA stores that
 // drain while the math warpgroups already run the next tile.  The split-K weight gradients leave the same way: each
 // unit's fp32 partial tile is added into dW by TMA reduce.  The generic epilogue loads and stores from registers.
+// The same kernel with FP8 = true is the e4m3 inference form (egovlp_gemm_e4m3): e4m3 operands with per-row scales of
+// A and per-column scales of B, applied in the staged epilogue.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -61,6 +63,9 @@ struct EpiParams {
   float* colsum;    // optional fp32 [N]: accumulates the column sums of the stored values (bias gradient)
   float* colsum_a;  // optional fp32 [M], MN-major A / MN-major B (wgrad) only: accumulates sum_k A[k, m], i.e. the bias
                     // gradient of the Linear whose weight gradient this GEMM computes, from the A tiles already in smem
+  // e4m3 operands only: acc[m, n] * row_scale[m] * w_scale[n] is the product, before the epilogue above
+  const float* row_scale;
+  const float* w_scale;
 };
 
 // Specialised epilogues stage through shared memory: each math warpgroup owns EPI_BUFS subtiles of 64 rows x 128 B
@@ -90,6 +95,42 @@ __device__ __forceinline__ void red_add_v2(float* p, float a, float b) {
   asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a), "f"(b) : "memory");
 }
 
+// wgmma accumulator operands: m64 x 256 (128 fp32 per thread) and m64 x 128 (64 per thread)
+#define WGMMA_ACC128 \
+  "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), \
+  "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), \
+  "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), \
+  "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), \
+  "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), \
+  "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), \
+  "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), \
+  "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), \
+  "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), \
+  "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), \
+  "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), \
+  "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), \
+  "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), \
+  "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), \
+  "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), \
+  "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+#define WGMMA_ACC64 \
+  "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), \
+  "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), \
+  "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), \
+  "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), \
+  "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), \
+  "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), \
+  "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), \
+  "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+#define WGMMA_REGS128 \
+  "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31," \
+  "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63," \
+  "%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95," \
+  "%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127"
+#define WGMMA_REGS64 \
+  "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31," \
+  "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63"
+
 // D (+)= A[smem desc] * B[smem desc], m64 x N x k16, bf16 -> fp32; TA / TB = 1 for an MN-major operand.
 template <int TA, int TB>
 __device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t adesc, uint64_t bdesc, int scale_d) {
@@ -97,27 +138,9 @@ __device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t adesc
       "{\n\t.reg .pred p;\n\t"
       "setp.ne.b32 p, %130, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
-      "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,"
-      "%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,"
-      "%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127}, "
+      "{" WGMMA_REGS128 "}, "
       "%128, %129, p, 1, 1, %131, %132;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
-        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
-        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
-        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
-        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
-        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
-        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : WGMMA_ACC128
       : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TA), "n"(TB));
 }
 template <int TA, int TB>
@@ -126,22 +149,38 @@ __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc,
       "{\n\t.reg .pred p;\n\t"
       "setp.ne.b32 p, %66, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
-      "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, "
+      "{" WGMMA_REGS64 "}, "
       "%64, %65, p, 1, 1, %67, %68;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : WGMMA_ACC64
       : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TA), "n"(TB));
 }
-template <int BLOCK_N, int TA, int TB>
+// the same for e4m3 x e4m3 -> fp32, m64 x N x k32: K-major operands only (the instruction has no transpose bits); one
+// k32 step reads 32 B of each operand row, as one bf16 k16 step does
+__device__ __forceinline__ void wgmma_m64n256k32_e4m3(float (&d)[128], uint64_t adesc, uint64_t bdesc, int scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k32.f32.e4m3.e4m3 "
+      "{" WGMMA_REGS128 "}, "
+      "%128, %129, p, 1, 1;\n\t}"
+      : WGMMA_ACC128
+      : "l"(adesc), "l"(bdesc), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_m64n128k32_e4m3(float (&d)[64], uint64_t adesc, uint64_t bdesc, int scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 "
+      "{" WGMMA_REGS64 "}, "
+      "%64, %65, p, 1, 1;\n\t}"
+      : WGMMA_ACC64
+      : "l"(adesc), "l"(bdesc), "r"(scale_d));
+}
+template <int BLOCK_N, int TA, int TB, bool FP8>
 __device__ __forceinline__ void wgmma_tile(float (&d)[BLOCK_N / 2], uint64_t adesc, uint64_t bdesc, int scale_d) {
-  if constexpr (BLOCK_N == 256) wgmma_m64n256k16<TA, TB>(d, adesc, bdesc, scale_d);
+  if constexpr (FP8 && BLOCK_N == 256) wgmma_m64n256k32_e4m3(d, adesc, bdesc, scale_d);
+  else if constexpr (FP8) wgmma_m64n128k32_e4m3(d, adesc, bdesc, scale_d);
+  else if constexpr (BLOCK_N == 256) wgmma_m64n256k16<TA, TB>(d, adesc, bdesc, scale_d);
   else wgmma_m64n128k16<TA, TB>(d, adesc, bdesc, scale_d);
 }
 
@@ -234,13 +273,19 @@ enum EpiMode {
   EPI_RED_F32 = 8,   // alpha -> fp32 add into out                                      (every wgrad)
 };
 
-template <int BLOCK_N, bool A_MN, bool B_MN, bool TWO, int MODE>
+// FP8: A and B are e4m3 (K-major both), one k-block = 128 elements = the same 128 B per row as a bf16 k-block, so the
+// TMA boxes, smem descriptors, stage ring and barriers are byte-identical; each k-block runs 4 k32 steps instead of 4
+// k16 steps, and the staged epilogue first multiplies the accumulators by the row and column scales.
+template <int BLOCK_N, bool A_MN, bool B_MN, bool TWO, int MODE, bool FP8>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                        const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmOut2,
                        const __grid_constant__ CUtensorMap tmIn, int M, int N, int K, int num_m_blocks,
                        int num_n_blocks, int kb_per_split, int num_splits, EpiParams ep) {
   static_assert(!(TWO && A_MN && B_MN), "the wgrad form (column sums of A) runs on single CTAs");
+  static_assert(!FP8 || (!A_MN && !B_MN && !TWO && (MODE == EPI_BF16 || MODE == EPI_ACT1)),
+                "e4m3: K-major operands, single CTAs, the qkv / fc1 inference epilogues");
+  constexpr int KB_ELEMS = FP8 ? 2 * BLOCK_K : BLOCK_K;      // elements of one 128-byte k-block row
   using C = Cfg<BLOCK_N>;
   constexpr int TILE_M = TWO ? 2 * BLOCK_M : BLOCK_M;
   const uint32_t rank = TWO ? cluster_ctarank() : 0u;      // CTA of the pair: rows 128 rank .. of the 256-row tile
@@ -278,7 +323,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
   const int lane = threadIdx.x & 31;
   const int num_tiles = num_m_blocks * num_n_blocks;
   const int num_units = num_tiles * num_splits;
-  const int num_kb = (K + BLOCK_K - 1) / BLOCK_K;
+  const int num_kb = (K + KB_ELEMS - 1) / KB_ELEMS;
   const bool sum_a = A_MN && B_MN && ep.colsum_a != nullptr;
 
   if (threadIdx.x == 0) {
@@ -326,7 +371,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
             mbar_expect_tx(fb, A_STAGE_BYTES + C::B_STAGE_BYTES);
             const uint32_t a_dst = sA + stage * A_STAGE_BYTES, b_dst = sB + stage * C::B_STAGE_BYTES;
             if (!A_MN) {
-              tma_load_2d(a_dst, &tmA, fb, kb * BLOCK_K, m_row);
+              tma_load_2d(a_dst, &tmA, fb, kb * KB_ELEMS, m_row);
             } else {
 #pragma unroll
               for (int i = 0; i < BLOCK_M / 64; ++i)
@@ -344,7 +389,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
                 }
               }
             } else if (!B_MN) {
-              tma_load_2d(b_dst, &tmB, fb, kb * BLOCK_K, n_row);
+              tma_load_2d(b_dst, &tmB, fb, kb * KB_ELEMS, n_row);
             } else {
 #pragma unroll
               for (int i = 0; i < BLOCK_N / 64; ++i)
@@ -469,7 +514,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
                                       : make_smem_desc_sw128(a_src + k * (WG_K * 2), 16, 1024);
           const uint64_t bdesc = B_MN ? make_smem_desc_sw128(b_src + k * (WG_K * 128), MN_ATOM_BYTES, 1024)
                                       : make_smem_desc_sw128(b_src + k * (WG_K * 2), 16, 1024);
-          wgmma_tile<BLOCK_N, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc, bdesc, (kb > kb0 || k > 0) ? 1 : 0);
+          wgmma_tile<BLOCK_N, A_MN ? 1 : 0, B_MN ? 1 : 0, FP8>(acc, adesc, bdesc, (kb > kb0 || k > 0) ? 1 : 0);
         }
         wgmma_commit();
         wgmma_fence_regs(acc);
@@ -493,6 +538,11 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
         // back to the input warp (or rewritten).  The global writes drain while the next subtile / tile runs.
         const int m_row = m_blk * TILE_M + (int)rank * BLOCK_M + mw * EPI_ROWS, n0 = n_blk * BLOCK_N;
         const int c2 = 2 * (lane & 3);
+        float rs[2] = {1.f, 1.f};             // FP8: the row scales of this thread's two rows (padding rows clamped)
+        if constexpr (FP8) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) rs[h] = __ldg(ep.row_scale + min(m_row + wq * 16 + (lane >> 2) + 8 * h, M - 1));
+        }
         if (!RED) mbar_wait_nocall(bias_full, tc & 1);
 #pragma unroll
         for (int s = 0; s < NSUB; ++s, ++it) {
@@ -508,14 +558,20 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
             float2 bq = make_float2(0.f, 0.f);
             if (!RED)
               asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(bq.x), "=f"(bq.y) : "r"(sBias + 4 * (8 * j + c2)));
+            float2 ws = make_float2(1.f, 1.f);        // FP8: column scales (N % 128 == 0: every column exists)
+            if constexpr (FP8) ws = __ldg(reinterpret_cast<const float2*>(ep.w_scale + n0 + 8 * j + c2));
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
               const int r = wq * 16 + (lane >> 2) + 8 * h;  // row of the subtile; 16-byte chunks XOR-swizzled by r & 7
               // bf16: chunk jj, 4 bytes per lane pair; fp32: chunk 2 jj + (lane % 4) / 2, 8 bytes per lane pair
               const uint32_t off = OUT_F32 ? r * 128 + (((2 * jj + ((lane & 3) >> 1)) ^ (r & 7)) << 4) + 8 * (lane & 1)
                                            : r * 128 + ((jj ^ (r & 7)) << 4) + 4 * (lane & 3);
-              float v0 = __fmaf_rn(acc[4 * j + 2 * h], ep.alpha, bq.x);
-              float v1 = __fmaf_rn(acc[4 * j + 2 * h + 1], ep.alpha, bq.y);
+              float a0 = acc[4 * j + 2 * h], a1 = acc[4 * j + 2 * h + 1];
+              if constexpr (FP8) {
+                a0 = __fmul_rn(__fmul_rn(a0, rs[h]), ws.x); a1 = __fmul_rn(__fmul_rn(a1, rs[h]), ws.y);
+              }
+              float v0 = __fmaf_rn(a0, ep.alpha, bq.x);
+              float v1 = __fmaf_rn(a1, ep.alpha, bq.y);
               if (MODE == EPI_BF16 && n0 + 8 * j + c2 < ep.col_scale_ncols) {
                 v0 = __fmul_rn(v0, ep.col_scale); v1 = __fmul_rn(v1, ep.col_scale);
               }
@@ -661,18 +717,24 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
   if (TWO) cluster_sync_all();      // the peer may still multicast into this CTA's smem or arrive on its barriers
 }
 
-template <int BLOCK_N, bool A_MN, bool B_MN, bool TWO, int MODE = EPI_GENERIC>
+template <int BLOCK_N, bool A_MN, bool B_MN, bool TWO, int MODE = EPI_GENERIC, bool FP8 = false>
 int launch(const void* A, long long lda, const void* B, long long ldb, int M, int N, int K, int splits,
            const EpiParams& ep, cudaStream_t stream) {
   using C = Cfg<BLOCK_N>;
   CUtensorMap tmA, tmB;
   int rc;
-  if (!A_MN) rc = make_tmap_2d_bf16(&tmA, A, M, K, lda, BLOCK_M, BLOCK_K);
-  else       rc = make_tmap_2d_bf16(&tmA, A, K, M, lda, BLOCK_K, 64);
-  if (rc) return rc;
-  if (!B_MN) rc = make_tmap_2d_bf16(&tmB, B, N, K, ldb, TWO ? BLOCK_N / 2 : BLOCK_N, BLOCK_K);
-  else       rc = make_tmap_2d_bf16(&tmB, B, K, N, ldb, BLOCK_K, 64);
-  if (rc) return rc;
+  if (FP8) {            // e4m3 bytes: the same [rows, 128 B] boxes as the K-major bf16 maps
+    rc = make_tmap_2d_u8(&tmA, A, M, K, lda, BLOCK_M, 2 * BLOCK_K);
+    if (!rc) rc = make_tmap_2d_u8(&tmB, B, N, K, ldb, BLOCK_N, 2 * BLOCK_K);
+    if (rc) return rc;
+  } else {
+    if (!A_MN) rc = make_tmap_2d_bf16(&tmA, A, M, K, lda, BLOCK_M, BLOCK_K);
+    else       rc = make_tmap_2d_bf16(&tmA, A, K, M, lda, BLOCK_K, 64);
+    if (rc) return rc;
+    if (!B_MN) rc = make_tmap_2d_bf16(&tmB, B, N, K, ldb, TWO ? BLOCK_N / 2 : BLOCK_N, BLOCK_K);
+    else       rc = make_tmap_2d_bf16(&tmB, B, K, N, ldb, BLOCK_K, 64);
+    if (rc) return rc;
+  }
   // epilogue subtiles of the staged forms: [64 rows, 128 B] boxes over out / out2 / residual / aux
   constexpr bool STAGED = MODE != EPI_GENERIC;
   CUtensorMap tmOut = {}, tmOut2 = {}, tmIn = {};
@@ -690,12 +752,12 @@ int launch(const void* A, long long lda, const void* B, long long ldb, int M, in
   constexpr int SMEM_BYTES = STAGED ? C::SMEM_BYTES_STAGED : C::SMEM_BYTES;
   constexpr int TILE_M = TWO ? 2 * BLOCK_M : BLOCK_M;
   const int num_m_blocks = (M + TILE_M - 1) / TILE_M, num_n_blocks = (N + BLOCK_N - 1) / BLOCK_N;
-  const int num_kb = (K + BLOCK_K - 1) / BLOCK_K;
+  const int num_kb = (K + (FP8 ? 2 : 1) * BLOCK_K - 1) / ((FP8 ? 2 : 1) * BLOCK_K);
   splits = max(1, min(splits, num_kb));
   const int kb_per_split = (num_kb + splits - 1) / splits;
   splits = (num_kb + kb_per_split - 1) / kb_per_split;  // no empty splits
   const int units = num_m_blocks * num_n_blocks * splits;
-  auto kern = gemm_bf16_wgmma_kernel<BLOCK_N, A_MN, B_MN, TWO, MODE>;
+  auto kern = gemm_bf16_wgmma_kernel<BLOCK_N, A_MN, B_MN, TWO, MODE, FP8>;
   static bool attr_set = false;
   if (!attr_set) {
     EGOVLP_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
@@ -833,6 +895,7 @@ extern "C" int egovlp_gemm_bf16(const void* A, int a_mn_major, long long lda, co
   ep.col_scale = e->col_scale; ep.col_scale_ncols = e->col_scale_ncols; ep.res_row_mod = e->res_row_mod;
   ep.colsum = e->colsum;
   ep.colsum_a = e->colsum_a;
+  ep.row_scale = ep.w_scale = nullptr;
   EGOVLP_CHECK_ARG(!e->colsum_a || (a_mn_major && b_mn_major && N % 256 == 0 && M % 8 == 0 &&
                                     (reinterpret_cast<uintptr_t>(e->colsum_a) & 15) == 0),
                    "gemm: colsum_a needs the MN/MN (wgrad) form with N % 256 == 0, M % 8 == 0 and a 16B-aligned vector");
@@ -841,4 +904,33 @@ extern "C" int egovlp_gemm_bf16(const void* A, int a_mn_major, long long lda, co
     return dispatch_mode<256, true>(a_mn_major, b_mn_major, A, lda, B, ldb, M, N, K, split_k, ep, st);
   if (N % 256 == 0) return dispatch_mode<256, false>(a_mn_major, b_mn_major, A, lda, B, ldb, M, N, K, split_k, ep, st);
   return dispatch_mode<128, false>(a_mn_major, b_mn_major, A, lda, B, ldb, M, N, K, split_k, ep, st);
+}
+
+extern "C" int egovlp_gemm_e4m3(const void* A8, long long lda, const void* B8, long long ldb, const float* row_scale,
+                                const float* col_scale, int M, int N, int K, const egovlp_gemm_epilogue* e,
+                                void* stream) {
+  EGOVLP_CHECK_ARG(A8 && B8 && row_scale && col_scale && e && e->out, "gemm_e4m3: null pointer");
+  EGOVLP_CHECK_ARG(M > 0 && N > 0 && K > 0 && N % 128 == 0 && K % 16 == 0,
+                   "gemm_e4m3: bad shape M=%d N=%d K=%d (N %% 128 == 0 and K %% 16 == 0 needed)", M, N, K);
+  EGOVLP_CHECK_ARG(lda >= K && ldb >= K && lda % 16 == 0 && ldb % 16 == 0,
+                   "gemm_e4m3: leading dimensions must be >= K and multiples of 16 (16B TMA strides)");
+  EGOVLP_CHECK_ARG(((reinterpret_cast<uintptr_t>(A8) | reinterpret_cast<uintptr_t>(B8) |
+                     reinterpret_cast<uintptr_t>(col_scale)) & 15) == 0,
+                   "gemm_e4m3: operands and column scales must be 16B aligned");
+  EGOVLP_CHECK_ARG(e->out_mode == 0 && (e->act == 0 || e->act == 1) && !e->residual && !e->aux && !e->out2 &&
+                       !e->colsum && !e->colsum_a && !e->res_row_mod && (e->act == 0 || e->col_scale_ncols == 0),
+                   "gemm_e4m3: only the bf16 store (act 0, optional column scale) and GELU (act 1) epilogues");
+  EGOVLP_CHECK_ARG(tma_ok(e->out, e->ldo * 2) && (reinterpret_cast<uintptr_t>(e->bias) & 15) == 0,
+                   "gemm_e4m3: out and bias must be 16B aligned, ldo a multiple of 8");
+  EpiParams ep = {};
+  ep.bias = e->bias; ep.out = e->out; ep.ldo = e->ldo; ep.out_mode = 0; ep.act = e->act; ep.alpha = e->alpha;
+  ep.col_scale = e->col_scale; ep.col_scale_ncols = e->col_scale_ncols;
+  ep.row_scale = row_scale; ep.w_scale = col_scale;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (N % 256 == 0) {
+    if (e->act == 1) return launch<256, false, false, false, EPI_ACT1, true>(A8, lda, B8, ldb, M, N, K, 1, ep, st);
+    return launch<256, false, false, false, EPI_BF16, true>(A8, lda, B8, ldb, M, N, K, 1, ep, st);
+  }
+  if (e->act == 1) return launch<128, false, false, false, EPI_ACT1, true>(A8, lda, B8, ldb, M, N, K, 1, ep, st);
+  return launch<128, false, false, false, EPI_BF16, true>(A8, lda, B8, ldb, M, N, K, 1, ep, st);
 }

@@ -13,12 +13,15 @@ constexpr int LN_WARPS = 8;
 
 // Forward: one row per warp, 8 rows per CTA (a persistent, register-prefetching variant measured slower: 36 % vs
 // 55 % of the HBM copy bandwidth at M = 50k rows -- occupancy beats explicit prefetch here).
-template <int NV>  // NV float4 per lane: covers D <= NV*128
+// Q8 (compile time, so that the other instantiations are unchanged): also y8 = the row in e4m3 with its scale in
+// row_scale (see e4m3_row_scale), from the fp32 values already in registers: the row amax is one more warp reduction.
+template <int NV, bool Q8>  // NV float4 per lane: covers D <= NV*128
 __global__ void __launch_bounds__(LN_WARPS * 32)
 layernorm_fwd_kernel(const float* __restrict__ x, long long ldx, const float* __restrict__ add,
                      float* __restrict__ sum_out, const float* __restrict__ gamma, const float* __restrict__ beta,
                      bf16* __restrict__ y16, float* __restrict__ y32, float* __restrict__ mean_out,
-                     float* __restrict__ rstd_out, int rows, int D, float eps) {
+                     float* __restrict__ rstd_out, int rows, int D, float eps, uint8_t* __restrict__ y8,
+                     float* __restrict__ row_scale) {
   const int row = blockIdx.x * LN_WARPS + (threadIdx.x >> 5);
   if (row >= rows) return;
   const int lane = threadIdx.x & 31;
@@ -58,6 +61,7 @@ layernorm_fwd_kernel(const float* __restrict__ x, long long ldx, const float* __
     if (mean_out) mean_out[row] = mean;
     if (rstd_out) rstd_out[row] = rstd;
   }
+  float amax = 0.f;
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
     const int c = (i * 32 + lane) * 4;
@@ -68,6 +72,22 @@ layernorm_fwd_kernel(const float* __restrict__ x, long long ldx, const float* __
       const float o2 = (v[i].z - mean) * rstd * g.z + b.z, o3 = (v[i].w - mean) * rstd * g.w + b.w;
       if (y16) *reinterpret_cast<uint2*>(y16 + (long long)row * D + c) = make_uint2(pack_bf16x2(o0, o1), pack_bf16x2(o2, o3));
       if (y32) *reinterpret_cast<float4*>(y32 + (long long)row * D + c) = make_float4(o0, o1, o2, o3);
+      if constexpr (Q8) {
+        v[i] = make_float4(o0, o1, o2, o3);
+        amax = fmaxf(amax, fmaxf(fmaxf(fabsf(o0), fabsf(o1)), fmaxf(fabsf(o2), fabsf(o3))));
+      }
+    }
+  }
+  if constexpr (Q8) {
+    float scale, inv;
+    e4m3_row_scale(warp_max(amax), scale, inv);
+    if (lane == 0) row_scale[row] = scale;
+#pragma unroll
+    for (int i = 0; i < NV; ++i) {
+      const int c = (i * 32 + lane) * 4;
+      if (c < D)
+        *reinterpret_cast<uint32_t*>(y8 + (long long)row * D + c) =
+            pack_e4m3x4(v[i].x * inv, v[i].y * inv, v[i].z * inv, v[i].w * inv);
     }
   }
 }
@@ -308,11 +328,12 @@ layernorm_bwd_pipe_kernel(const uint8_t* __restrict__ dy, int dy16, const float*
 
 constexpr int PIPE_FR = 8;         // forward: rows per tile = warps
 
-template <int NV>
+template <int NV, bool Q8>      // Q8: as layernorm_fwd_kernel
 __global__ void __launch_bounds__(PIPE_FR * 32, 2)
 layernorm_fwd_pipe_kernel(const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
                           bf16* __restrict__ y16, float* __restrict__ y32, float* __restrict__ mean_out,
-                          float* __restrict__ rstd_out, int rows, float eps) {
+                          float* __restrict__ rstd_out, int rows, float eps, uint8_t* __restrict__ y8,
+                          float* __restrict__ row_scale) {
   constexpr int D = NV * 128;
   constexpr uint32_t STAGE = PIPE_FR * D * 4;
   extern __shared__ __align__(128) uint8_t ln_smem[];
@@ -368,6 +389,7 @@ layernorm_fwd_pipe_kernel(const float* __restrict__ x, const float* __restrict__
         if (mean_out) mean_out[row] = mu;
         if (rstd_out) rstd_out[row] = rs;
       }
+      float amax = 0.f;
 #pragma unroll
       for (int i = 0; i < NV; ++i) {
         const long long off = (long long)row * D + (i * 32 + lane) * 4;
@@ -375,6 +397,19 @@ layernorm_fwd_pipe_kernel(const float* __restrict__ x, const float* __restrict__
         const float o2 = (v[i].z - mu) * rs * g4[i].z + b4[i].z, o3 = (v[i].w - mu) * rs * g4[i].w + b4[i].w;
         if (y16) *reinterpret_cast<uint2*>(y16 + off) = make_uint2(pack_bf16x2(o0, o1), pack_bf16x2(o2, o3));
         if (y32) *reinterpret_cast<float4*>(y32 + off) = make_float4(o0, o1, o2, o3);
+        if constexpr (Q8) {
+          v[i] = make_float4(o0, o1, o2, o3);
+          amax = fmaxf(amax, fmaxf(fmaxf(fabsf(o0), fabsf(o1)), fmaxf(fabsf(o2), fabsf(o3))));
+        }
+      }
+      if constexpr (Q8) {
+        float scale, inv;
+        e4m3_row_scale(warp_max(amax), scale, inv);
+        if (lane == 0) row_scale[row] = scale;
+#pragma unroll
+        for (int i = 0; i < NV; ++i)
+          *reinterpret_cast<uint32_t*>(y8 + (long long)row * D + (i * 32 + lane) * 4) =
+              pack_e4m3x4(v[i].x * inv, v[i].y * inv, v[i].z * inv, v[i].w * inv);
       }
     }
     __syncthreads();
@@ -445,24 +480,25 @@ colsum_kernel(const void* __restrict__ dy, long long ld, float* __restrict__ out
   }
 }
 
-template <int NV>
+template <int NV, bool Q8 = false>
 int launch_ln_fwd(const float* x, long long ldx, const float* add, float* sum_out, const float* gamma,
                   const float* beta, void* y16, float* y32, float* mean, float* rstd, int rows, int D, float eps,
-                  cudaStream_t st) {
+                  cudaStream_t st, uint8_t* y8 = nullptr, float* row_scale = nullptr) {
   if (ln_pipe_enabled() && D == NV * 128 && ldx == D && !add && !sum_out && rows >= 4096 && aligned16(x)) {
-    auto kern = layernorm_fwd_pipe_kernel<NV>;
+    auto kern = layernorm_fwd_pipe_kernel<NV, Q8>;
     const int smem = PIPE_STAGES * PIPE_FR * D * 4;
     static bool attr = false;
     if (!attr) { EGOVLP_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); attr = true; }
     const int tiles = (rows + PIPE_FR - 1) / PIPE_FR;
     kern<<<min(tiles, 2 * num_sms()), PIPE_FR * 32, smem, st>>>(x, gamma, beta, reinterpret_cast<bf16*>(y16), y32, mean, rstd,
-                                                                 rows, eps);
+                                                                 rows, eps, y8, row_scale);
     EGOVLP_CHECK_LAUNCH();
     return EGOVLP_OK;
   }
   const int grid = (rows + LN_WARPS - 1) / LN_WARPS;
-  layernorm_fwd_kernel<NV><<<grid, LN_WARPS * 32, 0, st>>>(x, ldx, add, sum_out, gamma, beta,
-                                                          reinterpret_cast<bf16*>(y16), y32, mean, rstd, rows, D, eps);
+  layernorm_fwd_kernel<NV, Q8><<<grid, LN_WARPS * 32, 0, st>>>(x, ldx, add, sum_out, gamma, beta,
+                                                              reinterpret_cast<bf16*>(y16), y32, mean, rstd, rows, D, eps,
+                                                              y8, row_scale);
   EGOVLP_CHECK_LAUNCH();
   return EGOVLP_OK;
 }
@@ -513,6 +549,23 @@ extern "C" int egovlp_layernorm_fwd(const float* x, long long ldx, const float* 
   return EGOVLP_ERR_UNSUPPORTED;
 }
 
+extern "C" int egovlp_layernorm_fwd_e4m3(const float* x, long long ldx, const float* gamma, const float* beta,
+                                         void* y_bf16, float* y_f32, float* mean, float* rstd, uint8_t* y8,
+                                         float* row_scale, int rows, int D, float eps, void* stream) {
+  EGOVLP_CHECK_ARG(x && gamma && beta && y8 && row_scale, "layernorm_fwd_e4m3: null pointer");
+  // D <= 256 is not instantiated: the D = 256 form spills (ptxas keeps it at 32 registers)
+  EGOVLP_CHECK_ARG(rows >= 0 && D > 256 && D % 4 == 0 && D <= 1024 && ldx % 4 == 0,
+                   "layernorm_fwd_e4m3: bad D=%d ldx=%lld (256 < D <= 1024, D %% 4 == 0)", D, ldx);
+  EGOVLP_CHECK_ARG((reinterpret_cast<uintptr_t>(y8) & 3) == 0, "layernorm_fwd_e4m3: y8 must be 4B aligned");
+  if (rows == 0) return EGOVLP_OK;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const int nv = (D + 127) / 128;
+#define LN_FWD8_CASE(n) case n: return launch_ln_fwd<n, true>(x, ldx, nullptr, nullptr, gamma, beta, y_bf16, y_f32, mean, rstd, rows, D, eps, st, y8, row_scale)
+  switch (nv) { LN_FWD8_CASE(3); LN_FWD8_CASE(4); LN_FWD8_CASE(5); LN_FWD8_CASE(6); LN_FWD8_CASE(7); LN_FWD8_CASE(8); }
+#undef LN_FWD8_CASE
+  return EGOVLP_ERR_UNSUPPORTED;
+}
+
 extern "C" int egovlp_layernorm_bwd(const void* dy, int dy_is_bf16, long long lddy, const float* x, long long ldx,
                                     const float* gamma, const float* mean, const float* rstd, const void* add1,
                                     int add1_is_bf16, const void* add2, int add2_is_bf16, float* dx, long long lddx,
@@ -538,6 +591,40 @@ extern "C" int egovlp_cast_f32_to_bf16(const float* src, void* dst_bf16, long lo
   if (g > (long long)num_sms() * 16) g = (long long)num_sms() * 16;
   const int grid = (int)g;
   cast_f32_to_bf16_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(src, reinterpret_cast<bf16*>(dst_bf16), n);
+  EGOVLP_CHECK_LAUNCH();
+  return EGOVLP_OK;
+}
+
+// One warp per row: the row amax, then the row in e4m3 with its scale (the weight operands of the e4m3 GEMM, one scale
+// per output channel).
+__global__ void quantize_rows_e4m3_kernel(const float* __restrict__ w, long long ldw, uint8_t* __restrict__ q,
+                                          float* __restrict__ scale, int rows, int K) {
+  const int row = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (row >= rows) return;
+  const float* wr = w + (long long)row * ldw;
+  float amax = 0.f;
+  for (int c = lane * 4; c < K; c += 128) {
+    const float4 v = *reinterpret_cast<const float4*>(wr + c);
+    amax = fmaxf(amax, fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))));
+  }
+  float s, inv;
+  e4m3_row_scale(warp_max(amax), s, inv);
+  if (lane == 0) scale[row] = s;
+  for (int c = lane * 4; c < K; c += 128) {
+    const float4 v = *reinterpret_cast<const float4*>(wr + c);
+    *reinterpret_cast<uint32_t*>(q + (long long)row * K + c) =
+        pack_e4m3x4(__fmul_rn(v.x, inv), __fmul_rn(v.y, inv), __fmul_rn(v.z, inv), __fmul_rn(v.w, inv));
+  }
+}
+
+extern "C" int egovlp_quantize_rows_e4m3(const float* w, long long ldw, uint8_t* q, float* scale, int rows, int K,
+                                         void* stream) {
+  EGOVLP_CHECK_ARG(w && q && scale && rows >= 0 && K > 0 && K % 4 == 0 && ldw >= K && ldw % 4 == 0,
+                   "quantize_rows_e4m3: bad args (K=%d ldw=%lld)", K, ldw);
+  EGOVLP_CHECK_ARG(((reinterpret_cast<uintptr_t>(w) & 15) | (reinterpret_cast<uintptr_t>(q) & 3)) == 0,
+                   "quantize_rows_e4m3: w must be 16B and q 4B aligned");
+  if (rows == 0) return EGOVLP_OK;
+  quantize_rows_e4m3_kernel<<<(rows + 7) / 8, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(w, ldw, q, scale, rows, K);
   EGOVLP_CHECK_LAUNCH();
   return EGOVLP_OK;
 }

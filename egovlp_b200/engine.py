@@ -75,10 +75,10 @@ except ImportError:                                           # pragma: no cover
 
 
 class _CastEntry:
-    __slots__ = ("ref", "t16", "version", "ptr", "gen", "trusted")
+    __slots__ = ("ref", "t16", "version", "ptr", "gen", "trusted", "scale")
 
-    def __init__(self, p, t16):
-        self.ref, self.t16 = weakref.ref(p), t16
+    def __init__(self, p, t16, scale=None):
+        self.ref, self.t16, self.scale = weakref.ref(p), t16, scale         # scale: e4m3 entries only
         self.version, self.ptr, self.gen, self.trusted = -1, 0, -1, False
 
     def stamp(self, p, trusted=False):
@@ -104,12 +104,15 @@ class Bf16Cache:
       optimizer generation changed (entries hold a weak reference, so a recycled `id()` cannot alias a dead parameter).
     * `refresh()` -- called at the top of every TRAINING forward -- re-casts every known copy in ONE launch
       (egovlp_cast_multi_f32_to_bf16) unless the fused AdamW just wrote it, so an update made through `p.data` by any
-      optimizer / EMA is always seen by the next training step."""
+      optimizer / EMA is always seen by the next training step.
+    * `get_e4m3(p)` returns (e4m3 [N, K], fp32 [N] per-row scales) of a 2-D weight for the fp8 inference GEMMs, under the
+      same invalidation rules; `refresh()` marks those entries stale, so they are re-quantised by the next fp8 forward."""
 
     def __init__(self):
         self._store = {}
         self._cats = {}
         self._table = None
+        self._e4m3 = {}
 
     def _entry(self, p, t16_factory):
         ent = self._store.get(id(p))
@@ -126,6 +129,17 @@ class Bf16Cache:
     def get(self, p, shape=None):
         t = self._entry(p, lambda: torch.empty(p.shape, dtype=BF16, device=p.device)).t16
         return t.view(shape) if shape is not None else t
+
+    def get_e4m3(self, p):
+        ent = self._e4m3.get(id(p))
+        if ent is None or ent.ref() is not p or ent.t16.device != p.device:
+            ent = _CastEntry(p, torch.empty(p.shape, dtype=ops.E4M3, device=p.device),
+                             torch.empty(p.shape[0], dtype=F32, device=p.device))
+            self._e4m3[id(p)] = ent
+        if not ent.current(p):
+            ops.quantize_rows_e4m3(p.detach().contiguous(), ent.t16, ent.scale)
+            ent.stamp(p)
+        return ent.t16, ent.scale
 
     def cat(self, name, params):
         """bf16 concat along dim 0 of several parameters (DistilBERT q/k/v -> one [3D, D] operand): every part is a cache
@@ -146,6 +160,11 @@ class Bf16Cache:
 
     def refresh(self):
         """Bring every cached copy up to date with one multi-tensor cast (no-op for copies the fused AdamW just wrote)."""
+        for key, ent in list(self._e4m3.items()):
+            if ent.ref() is None:
+                del self._e4m3[key]
+            else:
+                ent.version = -1
         live = []
         for key, ent in list(self._store.items()):
             p = ent.ref()
@@ -172,6 +191,7 @@ class Bf16Cache:
                 del _SHADOWS[key]
         self._store.clear()
         self._cats.clear()
+        self._e4m3.clear()
         self._table = None
 
 
@@ -359,6 +379,14 @@ def _ln16(inp, w, b, eps):
     return y, mean, rstd
 
 
+def _ln8(inp, w, b, eps):
+    """-> ((e4m3 LayerNorm(inp), its per-row scales), None, None): the A operand of the fp8 inference GEMMs."""
+    M, D = inp.shape
+    y8, scale = _empty((M, D), ops.E4M3, inp), _empty((M,), F32, inp)
+    ops.layernorm_fwd(inp, w.detach(), b.detach(), eps, y8=y8, row_scale=scale)
+    return (y8, scale), None, None
+
+
 def _proj_residual(a, pw, pb, resid, cache):
     """fp32 resid + proj(a): the attention output projection on the bias + fp32 residual GEMM form."""
     out = _empty(resid.shape, F32, a)
@@ -371,7 +399,10 @@ class SpaceTimeBlockFn(torch.autograd.Function):
 
     params: norm1.{w,b}, attn.qkv.{w,b}, attn.proj.{w,b}, timeattn.qkv.{w,b}, timeattn.proj.{w,b},
             norm2.{w,b}, mlp.fc1.{w,b}, mlp.fc2.{w,b}, norm3.{w,b}      (18 tensors, reference order)
-    dims: (B, T, N, H, grad_mode, low_memory).  low_memory = selective activation recompute for training: the forward
+    dims: (B, T, N, H, grad_mode, low_memory, fp8).  fp8 = e4m3 inference (set_inference_precision): a forward that
+    records no autograd runs the qkv and fc1 GEMMs on e4m3 operands -- the LayerNorm writes its output as e4m3 with
+    per-row scales, the weights come per-output-channel scaled from the cache; a training forward ignores the flag (the
+    backward needs the bf16 operands).  low_memory = selective activation recompute for training: the forward
     saves x, qkv, the attention outputs, the softmax and LayerNorm statistics and the bf16 fc1 pre-activation z (21,624
     instead of 38,520 bytes per token at D = 768); the backward rebuilds the residuals tr / sr and the LayerNorm outputs
     from them with the forward's own kernels (bit-identical), and GELU(z) / GELU'(z) inside the fc2 input-gradient GEMM.
@@ -380,7 +411,7 @@ class SpaceTimeBlockFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, dims, eps, cache, *p):
         (n1w, n1b, sqw, sqb, spw, spb, tqw, tqb, tpw, tpb, n2w, n2b, f1w, f1b, f2w, f2b, n3w, n3b) = p
-        B, T, N, H, grad_mode, low_memory = dims
+        B, T, N, H, grad_mode, low_memory, fp8 = dims
         D = H * 64
         S = 1 + T * N
         M = B * S
@@ -389,24 +420,32 @@ class SpaceTimeBlockFn(torch.autograd.Function):
         # `grad_mode` = torch.is_grad_enabled() at the call site: inside Function.forward grad mode is always off and
         # needs_input_grad reflects requires_grad of the parameters even under torch.no_grad()
         train = grad_mode and any(ctx.needs_input_grad)
+        fp8 = fp8 and not train
+        ln = _ln8 if fp8 else _ln16
 
-        def attention(inp16, qw, qb, pw, pb, mode, resid):
-            qkv = _empty((M, 3 * D), BF16, inp16)
-            ops.gemm(inp16, cache.get(qw), qkv, bias=qb.detach(), col_scale=Q_SCALE, col_scale_ncols=D)
+        def attention(inp, qw, qb, pw, pb, mode, resid):
+            qkv = _empty((M, 3 * D), BF16, x2)
+            if fp8:
+                ops.gemm_e4m3(*inp, *cache.get_e4m3(qw), qkv, bias=qb.detach(), col_scale=Q_SCALE, col_scale_ncols=D)
+            else:
+                ops.gemm(inp, cache.get(qw), qkv, bias=qb.detach(), col_scale=Q_SCALE, col_scale_ncols=D)
             a, lse = ops.divided_attn_fwd(qkv, B, T, N, H, mode)
             return qkv, a, lse, _proj_residual(a, pw, pb, resid, cache)
 
-        n3, mean3, rstd3 = _ln16(x2, n3w, n3b, eps)
+        n3, mean3, rstd3 = ln(x2, n3w, n3b, eps)
         qkv_t, a_t, lse_t, tr = attention(n3, tqw, tqb, tpw, tpb, 0, x2)          # time_residual = x + time_output
-        n1, mean1, rstd1 = _ln16(tr, n1w, n1b, eps)
+        n1, mean1, rstd1 = ln(tr, n1w, n1b, eps)
         qkv_s, a_s, lse_s, sr = attention(n1, sqw, sqb, spw, spb, 1, x2)          # space_residual = x + space_output
-        n2, mean2, rstd2 = _ln16(sr, n2w, n2b, eps)
+        n2, mean2, rstd2 = ln(sr, n2w, n2b, eps)
         h = _empty((M, HID), BF16, x2)
         # training: u = GELU'(fc1 output) for the backward, or in the low-memory mode z = the fc1 output itself (act 1
         # with out2: h is bit-identical to act 3's)
         u = _empty((M, HID), BF16, x2) if train else None
         act = (1 if low_memory else _ACT_FWD) if train else 1
-        ops.gemm(n2, cache.get(f1w), h, bias=f1b.detach(), act=act, out2=u)
+        if fp8:
+            ops.gemm_e4m3(*n2, *cache.get_e4m3(f1w), h, bias=f1b.detach(), act=1)
+        else:
+            ops.gemm(n2, cache.get(f1w), h, bias=f1b.detach(), act=act, out2=u)
         y = _empty((M, D), F32, x2)
         ops.gemm(h, cache.get(f2w), y, bias=f2b.detach(), residual=sr)
         if train:

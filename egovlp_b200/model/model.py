@@ -68,6 +68,8 @@ def _build_video_tower(video_params, from_scratch):
     tower.head = tower.pre_logits = tower.fc = nn.Identity()      # `fc`: "backwards compatibility (old models)"
     # selective activation recompute in training (a key the reference does not read: its configs load unchanged there)
     tower.set_grad_checkpointing(bool(video_params.get('grad_checkpointing', False)))
+    # e4m3 inference GEMMs, opt-in (another key the reference does not read)
+    tower.set_inference_precision(video_params.get('inference_precision', 'bf16'))
     if from_scratch:
         if os.path.exists(_VIT_B16_FILE):
             vit = torch.load(_VIT_B16_FILE, map_location="cpu")

@@ -87,14 +87,15 @@ class SpaceTimeBlock(nn.Module):
                 self.mlp.fc2.weight, self.mlp.fc2.bias, self.norm3.weight, self.norm3.bias)
 
     def forward(self, x, einops_from_space=None, einops_to_space=None, einops_from_time=None, einops_to_time=None,
-                time_n=None, space_f=None, cache=None, low_memory=False):
+                time_n=None, space_f=None, cache=None, low_memory=False, fp8=False):
         """x [B, 1 + space_f*time_n, D] fp32.  The einops pattern arguments of the reference signature are
         accepted and ignored: the token layout is fixed to the reference's 'b (f n) d'.  `low_memory`: selective
-        activation recompute in training (see SpaceTimeTransformer.set_grad_checkpointing)."""
+        activation recompute in training (see SpaceTimeTransformer.set_grad_checkpointing); `fp8`: e4m3 inference GEMMs
+        (see SpaceTimeTransformer.set_inference_precision)."""
         B = x.shape[0]
         eps = self.norm1.eps
         cache = cache if cache is not None else _default_cache(self)
-        dims = (B, space_f, time_n, self.num_heads, torch.is_grad_enabled(), bool(low_memory))
+        dims = (B, space_f, time_n, self.num_heads, torch.is_grad_enabled(), bool(low_memory), bool(fp8))
         return engine.SpaceTimeBlockFn.apply(x, dims, eps, cache, *self.kernel_params())
 
 
@@ -152,6 +153,7 @@ class SpaceTimeTransformer(nn.Module):
         self.einops_from_space, self.einops_to_space = 'b (f n) d', '(b f) n d'
         self.einops_from_time, self.einops_to_time = 'b (f n) d', '(b n) f d'
         self.grad_checkpointing = False
+        self.inference_precision = "bf16"
         object.__setattr__(self, "_bf16_cache", engine.Bf16Cache())
 
     def set_grad_checkpointing(self, enable=True):
@@ -161,6 +163,19 @@ class SpaceTimeTransformer(nn.Module):
         LayerNorm outputs and GELU / GELU' of the pre-activation from them.  The forward, inference and the state_dict
         are unchanged; the MLP gradients are rounded slightly differently (GELU is taken of the bf16 pre-activation)."""
         self.grad_checkpointing = bool(enable)
+
+    def set_inference_precision(self, precision="bf16"):
+        """Trade a bounded accuracy loss for speed in inference.  "fp8": forwards that record no autograd (evaluation,
+        feature extraction under torch.no_grad()) run each block's three LayerNorm-fed GEMMs -- timeattn.qkv, attn.qkv
+        and mlp.fc1, 62.5 % of the block's GEMM FLOPs -- on e4m3 tensor-core operands: the LayerNorm output with one
+        scale per token row, the weights with one scale per output channel (re-quantised whenever the parameter
+        changes).  Rows stay independent, so results do not depend on the batch size.  Every other GEMM, the text
+        tower, and every training forward of the tower (grad mode on and a parameter or input of a block requiring a
+        gradient) stay bf16; a tower frozen with requires_grad_(False) runs in fp8 even while a head on top trains.  "bf16" (the
+        default) restores the bf16 path bit for bit.  The state_dict is unchanged."""
+        if precision not in ("bf16", "fp8"):
+            raise ValueError(f"inference precision must be 'bf16' or 'fp8', got {precision!r}")
+        self.inference_precision = precision
 
     def forward_tokens(self, x, _refresh=True):
         """All tokens after the 12 blocks, [B, S, D] fp32 (before the final norm)."""
@@ -176,7 +191,8 @@ class SpaceTimeTransformer(nn.Module):
                                       pe.proj.bias, cache, getattr(self, "input_norm", None))
         n = (H // pe.patch_size[0]) * (W // pe.patch_size[1])
         for blk in self.blocks:
-            x = blk(x, time_n=n, space_f=F, cache=cache, low_memory=self.grad_checkpointing)
+            x = blk(x, time_n=n, space_f=F, cache=cache, low_memory=self.grad_checkpointing,
+                    fp8=self.inference_precision == "fp8")
         return x
 
     def forward_features(self, x, proj=None, _refresh=True):

@@ -6,7 +6,7 @@ import torch
 
 from ._lib import GemmEpilogue, call, lib
 
-BF16, F32 = torch.bfloat16, torch.float32
+BF16, F32, E4M3 = torch.bfloat16, torch.float32, torch.float8_e4m3fn
 
 
 def _ptr(t):
@@ -111,15 +111,27 @@ def gemm(a, b, out, *, a_mn=False, b_mn=False, bias=None, residual=None, aux=Non
     return out
 
 
-def layernorm_fwd(x, gamma, beta, eps, *, add=None, sum_out=None, y16=None, y32=None, mean=None, rstd=None):
-    """x fp32 [rows, D] (row stride free).  Returns nothing; writes the provided outputs."""
+def layernorm_fwd(x, gamma, beta, eps, *, add=None, sum_out=None, y16=None, y32=None, mean=None, rstd=None, y8=None,
+                  row_scale=None):
+    """x fp32 [rows, D] (row stride free).  Returns nothing; writes the provided outputs.  y8 (float8_e4m3fn [rows, D])
+    with row_scale (fp32 [rows]): the output as the A operand of `gemm_e4m3` (no `add` / `sum_out` then)."""
     _chk(x, F32, "x")
     rows, D = x.shape
     assert x.stride(1) == 1
     for t in (add, sum_out, y32):
         assert t is None or (t.dtype == F32 and t.is_contiguous() and t.shape == (rows, D))
     assert y16 is None or (y16.dtype == BF16 and y16.is_contiguous() and y16.shape == (rows, D))
-    nbytes = rows * D * (4 + 4 * (add is not None) + 4 * (sum_out is not None) + 2 * (y16 is not None) + 4 * (y32 is not None))
+    assert (y8 is None) == (row_scale is None), "y8 and row_scale go together"
+    nbytes = rows * D * (4 + 4 * (add is not None) + 4 * (sum_out is not None) + 2 * (y16 is not None) + 4 * (y32 is not None)
+                         + (y8 is not None))
+    if y8 is not None:
+        assert add is None and sum_out is None
+        _chk(y8, E4M3, "y8"); _chk(row_scale, F32, "row_scale")
+        assert y8.is_contiguous() and y8.shape == (rows, D) and row_scale.is_contiguous() and row_scale.numel() == rows
+        with _Probe("layernorm_fwd", nbytes):
+            call("egovlp_layernorm_fwd_e4m3", _ptr(x), C.c_longlong(x.stride(0)), _ptr(gamma), _ptr(beta), _ptr(y16),
+                 _ptr(y32), _ptr(mean), _ptr(rstd), _ptr(y8), _ptr(row_scale), rows, D, C.c_float(eps), _stream())
+        return
     with _Probe("layernorm_fwd", nbytes):
         call("egovlp_layernorm_fwd", _ptr(x), C.c_longlong(x.stride(0)), _ptr(add), _ptr(sum_out), _ptr(gamma),
              _ptr(beta), _ptr(y16), _ptr(y32), _ptr(mean), _ptr(rstd), rows, D, C.c_float(eps), _stream())
@@ -143,6 +155,40 @@ def layernorm_bwd(dy, x, gamma, mean, rstd, *, add1=None, add2=None, dx=None, dx
              int(add1 is not None and add1.dtype == BF16), _ptr(add2), int(add2 is not None and add2.dtype == BF16),
              _ptr(dx), C.c_longlong(dx.stride(0) if dx is not None else D), _ptr(dx16), _ptr(dgamma), _ptr(dbeta),
              _ptr(colsum_dx), rows, D, _stream())
+
+
+def gemm_e4m3(a8, a_scale, b8, b_scale, out, *, bias=None, act=0, alpha=1.0, col_scale=1.0, col_scale_ncols=0):
+    """out bf16 [M, N] = epi((a8 @ b8^T) * a_scale[:, None] * b_scale[None, :]); a8 [M, K] / b8 [N, K] float8_e4m3fn,
+    K-major; epi = bias, then the column scale (act 0) or GELU (act 1) -- see egovlp_gemm_e4m3."""
+    _chk(a8, E4M3, "a8"); _chk(b8, E4M3, "b8"); _chk(a_scale, F32, "a_scale"); _chk(b_scale, F32, "b_scale")
+    _chk(out, BF16, "out")
+    assert a8.dim() == 2 and b8.dim() == 2 and a8.stride(1) == 1 and b8.stride(1) == 1
+    (M, K), (N, Kb) = a8.shape, b8.shape
+    assert K == Kb and out.shape == (M, N) and out.stride(1) == 1, (a8.shape, b8.shape, out.shape)
+    assert a_scale.is_contiguous() and a_scale.numel() == M and b_scale.is_contiguous() and b_scale.numel() == N
+    e = GemmEpilogue()
+    if bias is not None:
+        _chk(bias, F32, "bias"); assert bias.numel() == N
+        e.bias = bias.data_ptr()
+    e.out, e.ldo, e.out_mode = out.data_ptr(), out.stride(0), 0
+    e.act, e.alpha, e.col_scale, e.col_scale_ncols = act, alpha, col_scale, col_scale_ncols
+    with _Probe("gemm_e4m3", 2.0 * M * N * K):
+        call("egovlp_gemm_e4m3", _ptr(a8), C.c_longlong(a8.stride(0)), _ptr(b8), C.c_longlong(b8.stride(0)),
+             _ptr(a_scale), _ptr(b_scale), M, N, K, C.byref(e), _stream())
+    return out
+
+
+def quantize_rows_e4m3(w, q=None, scale=None):
+    """fp32 [N, K] -> (float8_e4m3fn [N, K], fp32 [N] per-row scales), see egovlp_quantize_rows_e4m3."""
+    _chk(w, F32, "w")
+    assert w.dim() == 2 and w.stride(1) == 1
+    N, K = w.shape
+    q = torch.empty(N, K, dtype=E4M3, device=w.device) if q is None else q
+    scale = torch.empty(N, dtype=F32, device=w.device) if scale is None else scale
+    _chk(q, E4M3, "q"); _chk(scale, F32, "scale")
+    assert q.is_contiguous() and q.shape == (N, K) and scale.is_contiguous() and scale.numel() == N
+    call("egovlp_quantize_rows_e4m3", _ptr(w), C.c_longlong(w.stride(0)), _ptr(q), _ptr(scale), N, K, _stream())
+    return q, scale
 
 
 def cast_bf16(src, dst=None):

@@ -74,6 +74,15 @@ typedef struct egovlp_gemm_epilogue {
 
 int egovlp_gemm_bf16(const void* A, int a_mn_major, long long lda, const void* B, int b_mn_major, long long ldb,
                      int M, int N, int K, const egovlp_gemm_epilogue* epi, int split_k, void* stream);
+/* e4m3 inference form of the same GEMM (the video tower's LayerNorm-fed qkv and Mlp.fc1 GEMMs, opt-in,
+ * SpaceTimeTransformer.set_inference_precision("fp8")):
+ *   D[m,n] = epi( (sum_k A8[m,k] * B8[n,k]) * row_scale[m] * col_scale[n] )
+ * A8 [M, lda] and B8 [N, ldb] are e4m3 (e4m3fn bytes), both K-major; row_scale fp32 [M], col_scale fp32 [N] (16B
+ * aligned).  fp32 accumulation in the e4m3 wgmma.  Only two epilogues: act 0 with out_mode 0 (bias, optional column
+ * scale, bf16 out; the qkv form) and act 1 with out_mode 0 (bias, GELU, bf16 out; fc1).  No residual, aux, out2, column
+ * sums or split-K.  Constraints: N % 128 == 0, K % 16 == 0, lda / ldb >= K and multiples of 16, 16B-aligned bases. */
+int egovlp_gemm_e4m3(const void* A8, long long lda, const void* B8, long long ldb, const float* row_scale,
+                     const float* col_scale, int M, int N, int K, const egovlp_gemm_epilogue* epi, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * LayerNorm over the last dim (nn.LayerNorm; model/video_transformer.py:146,156,159,228,253 eps 1e-6;
@@ -85,6 +94,13 @@ int egovlp_gemm_bf16(const void* A, int a_mn_major, long long lda, const void* B
 int egovlp_layernorm_fwd(const float* x, long long ldx, const float* add, float* sum_out, const float* gamma,
                          const float* beta, void* y_bf16, float* y_f32, float* mean, float* rstd, int rows, int D,
                          float eps, void* stream);
+/* The same forward (no fused add) that also writes the normalised row as the A operand of egovlp_gemm_e4m3:
+ * y8 e4m3 [rows, D] (contiguous, 4B aligned) = y * (448 / amax) rounded to nearest with saturation, row_scale fp32
+ * [rows] = amax / 448, amax = max |y| over the row of fp32 outputs (scale 1 for a row of zeros).  y_bf16 / y_f32 /
+ * mean / rstd may each be NULL and are bit-identical to egovlp_layernorm_fwd's.  256 < D <= 1024. */
+int egovlp_layernorm_fwd_e4m3(const float* x, long long ldx, const float* gamma, const float* beta, void* y_bf16,
+                              float* y_f32, float* mean, float* rstd, uint8_t* y8, float* row_scale, int rows, int D,
+                              float eps, void* stream);
 /* Backward.  dx = LNbwd(dy) [+ add1] [+ add2]  (fp32 [rows, D], row stride lddx), optionally also stored as bf16
  * (dx_bf16, row stride D) for use as a GEMM operand.  add1/add2 carry the residual-stream gradients that bypass the LN
  * (SpaceTimeBlock: dsr = dy + LN2bwd, dx = dsr + dtr + LN3bwd).  dgamma/dbeta (fp32 [D]) are ACCUMULATED
@@ -312,6 +328,10 @@ int egovlp_gt_ranks(const void* sims, int is_f64, long long ld, int rows, int co
  */
 /* fp32 -> bf16 cast (weights: fp32 master -> bf16 GEMM operand). */
 int egovlp_cast_f32_to_bf16(const float* src, void* dst_bf16, long long n, void* stream);
+/* Per-row e4m3 quantisation of fp32 weights W [rows, K] (row stride ldw) for egovlp_gemm_e4m3: scale[r] = amax_r / 448
+ * (1 for a zero row), q [rows, K] contiguous = e4m3(W[r, k] * (448 / amax_r)), round to nearest, saturating.  K % 4 == 0,
+ * w 16B and q 4B aligned. */
+int egovlp_quantize_rows_e4m3(const float* w, long long ldw, uint8_t* q, float* scale, int rows, int K, void* stream);
 /* out[n] += sum_m dy[m, n]  (bias gradients).  dy bf16 or fp32 [M, N] row stride ld. */
 int egovlp_colsum_accum(const void* dy, int dy_is_fp32, long long ld, float* out, int M, int N, void* stream);
 
