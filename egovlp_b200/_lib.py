@@ -38,7 +38,7 @@ def lib():
 # kernels launched per C-ABI call (memsets excluded) -- bench.py reports the count as `gpu_launches`
 _KERNELS_PER_CALL = {"egovlp_egonce_fused_max_g": 0, "egovlp_divided_attn_fwd": 2, "egovlp_divided_attn_bwd": 2, "egovlp_video_embed_bwd": 2,
                      "egovlp_nce_fwd": 2, "egovlp_dual_softmax": 2, "egovlp_cross_entropy_fwd": 2,
-                     "egovlp_narrow_linear_bwd": 3}
+                     "egovlp_narrow_linear_bwd": 3, "egovlp_text_attn_long_bwd": 3}
 _launches = 0
 
 

@@ -42,35 +42,6 @@ struct Geom {
   int gsize;                // rows per group id (space: N, time: T)
 };
 
-__device__ __forceinline__ uint32_t sw_addr(uint32_t base, int row, int chunk) {
-  return base + row * ROW_BYTES + ((chunk ^ (row & 7)) << 4);
-}
-__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void ldsm_x4_t(uint32_t addr, uint32_t (&r)[4]) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void mma_bf16(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-// A-operand fragment (16 rows x 16 k) of a swizzled [rows x 64] tile: rows r0.., k-step kk
-__device__ __forceinline__ void load_a_frag(uint32_t tile, int r0, int kk, int lane, uint32_t (&f)[4]) {
-  ldsm_x4(sw_addr(tile, r0 + (lane & 7) + ((lane >> 3) & 1) * 8, kk * 2 + (lane >> 4)), f);
-}
-// B-operand fragments for two 8-wide n-tiles (n = rows n0..n0+15 of the tile, k = its 64 columns), k-step kk
-__device__ __forceinline__ void load_b_frag_nk(uint32_t tile, int n0, int kk, int lane, uint32_t (&f)[4]) {
-  ldsm_x4(sw_addr(tile, n0 + (lane & 7) + (lane >> 4) * 8, kk * 2 + ((lane >> 3) & 1)), f);
-}
-// B-operand fragments with k = rows k0..k0+15 of the tile, n = columns dp*16..dp*16+15 (two n-tiles), transposed load
-__device__ __forceinline__ void load_b_frag_kn(uint32_t tile, int k0, int dp, int lane, uint32_t (&f)[4]) {
-  ldsm_x4_t(sw_addr(tile, k0 + (lane & 7) + ((lane >> 3) & 1) * 8, dp * 2 + (lane >> 4)), f);
-}
-
 // token (0..S-1) held by smem row r of group g, or -1 for padding / out-of-range patches
 __device__ __forceinline__ int row_token(const Geom& G, int g, int r) {
   if (r == G.NP) return 0;

@@ -15,6 +15,7 @@ import weakref
 import torch
 
 from . import ops
+from ._lib import EgovlpError
 
 BF16, F32 = torch.bfloat16, torch.float32
 Q_SCALE = 0.125            # head_dim ** -0.5 for head_dim = 64 (model/video_transformer.py:87)
@@ -607,6 +608,11 @@ class ClsHeadFn(torch.autograd.Function):
 # ----------------------------------------------------------------------------------------------------------
 # text tower (DistilBERT) + ReLU/Linear projection
 # ----------------------------------------------------------------------------------------------------------
+# Longest caption the one-CTA-per-(sample, head) text attention (text_attn_*) takes; longer ones, up to the 512
+# positions of DistilBERT, run the tiled kernel (text_attn_long_*), which also keeps the rows' lse for the backward.
+TEXT_ATTN_SHORT_MAX_L = 128
+
+
 class TextTowerFn(torch.autograd.Function):
     """DistilBertModel(...).last_hidden_state -> (CLS | all tokens) -> ReLU -> Linear  (model/model.py:117-138).
 
@@ -629,13 +635,17 @@ class TextTowerFn(torch.autograd.Function):
         pw, pb = p[-2:]
         layers = [p[4 + 16 * i: 4 + 16 * (i + 1)] for i in range((len(p) - 6) // 16)]
         B, L = input_ids.shape
+        if L > pos.shape[0]:
+            raise EgovlpError(f"text tower: sequence length {L} exceeds the {pos.shape[0]} position embeddings "
+                              "(max_position_embeddings); truncate the captions to that length")
         D = word.shape[1]
         M = B * L
+        long_attn = L > TEXT_ATTN_SHORT_MAX_L
         ids = input_ids.contiguous().to(torch.int64)
         mask = attention_mask.contiguous().to(torch.int64)
         dev = word
         train = grad_mode and any(ctx.needs_input_grad)
-        saved = []
+        saved, lses = [], []
         p_hid, p_att = (float(drop[0]), float(drop[1])) if drop else (0.0, 0.0)
         seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if (p_hid > 0 or p_att > 0) else 0
 
@@ -655,7 +665,12 @@ class TextTowerFn(torch.autograd.Function):
             qkv = _empty((M, 3 * D), BF16, dev)
             ops.gemm(x16, wqkv, qkv, bias=bqkv, col_scale=Q_SCALE, col_scale_ncols=D)
             ctxv = _empty((M, D), BF16, dev)
-            ops.text_attn_fwd(qkv, mask, ctxv, B, L, heads, p_att, seed, 1 + 2 * li)
+            if long_attn:
+                lse = _empty((B, heads, L), F32, dev)
+                ops.text_attn_long_fwd(qkv, mask, ctxv, lse, B, L, heads, p_att, seed, 1 + 2 * li)
+                lses.append(lse)
+            else:
+                ops.text_attn_fwd(qkv, mask, ctxv, B, L, heads, p_att, seed, 1 + 2 * li)
             sa = _empty((M, D), F32, dev)
             ops.gemm(ctxv, cache.get(ow), sa, bias=ob.detach(), residual=x)               # sa_output + x
             x1, x1_16 = _empty((M, D), F32, dev), _empty((M, D), BF16, dev)
@@ -687,7 +702,8 @@ class TextTowerFn(torch.autograd.Function):
             ctx.meta = (B, L, D, heads, tokens_mode, len(layers), len(saved), p_hid, p_att, seed)
             ctx.cache = cache
             ctx.has_proj = pw is not None
-            ctx.save_for_backward(ids, mask, x, r16, *saved, *p[:len(p) - (0 if pw is not None else 2)])
+            ctx.n_lse = len(lses)
+            ctx.save_for_backward(ids, mask, x, r16, *saved, *lses, *p[:len(p) - (0 if pw is not None else 2)])
         return out.view(B, L, -1) if tokens_mode else out
 
     @staticmethod
@@ -697,7 +713,8 @@ class TextTowerFn(torch.autograd.Function):
         sv = ctx.saved_tensors
         ids, mask, x_last, r16 = sv[:4]
         saved = list(sv[4:4 + n_saved])
-        p = sv[4 + n_saved:]
+        lses = sv[4 + n_saved:4 + n_saved + ctx.n_lse]          # one per layer when L > TEXT_ATTN_SHORT_MAX_L
+        p = sv[4 + n_saved + ctx.n_lse:]
         word, pos, elw, elb = p[:4]
         layers = [p[4 + 16 * i: 4 + 16 * (i + 1)] for i in range(n_layers)]
         M = B * L
@@ -742,7 +759,11 @@ class TextTowerFn(torch.autograd.Function):
             dctx = _empty((M, D), BF16, dout)
             ops.gemm(dsa16, cache.get(ow), dctx, b_mn=True)
             dqkv = _empty((M, 3 * D), BF16, dout)
-            ops.text_attn_bwd(qkv, mask, dctx, dqkv, B, L, heads, Q_SCALE, p_att, seed, 1 + 2 * li)
+            if lses:
+                ops.text_attn_long_bwd(qkv, mask, ctxv, lses[li], dctx, dqkv, B, L, heads, Q_SCALE, p_att, seed,
+                                       1 + 2 * li)
+            else:
+                ops.text_attn_bwd(qkv, mask, dctx, dqkv, B, L, heads, Q_SCALE, p_att, seed, 1 + 2 * li)
             g_wqkv, g_bqkv = wgrad(dqkv, x16, 3 * D, D), bgrad(dqkv)
             wqkv = cache.cat(("text_qkv_w", li, id(qw)), (qw, kw, vw))
             dxin = _empty((M, D), F32, dout)

@@ -364,6 +364,23 @@ def text_attn_bwd(qkv, mask, dout, dqkv, B, L, H, q_scale, p_drop=0.0, seed=0, s
          C.c_float(p_drop), C.c_ulonglong(seed), C.c_uint(site), _stream())
 
 
+def text_attn_long_fwd(qkv, mask, out, lse, B, L, H, p_drop=0.0, seed=0, site=0):
+    """Tiled text attention (L <= 512): out bf16 [B*L, H*64], lse fp32 [B, H, L] (kept for the backward)."""
+    assert mask.dtype == torch.int64 and mask.is_contiguous()
+    _chk(lse, F32, "lse")
+    assert lse.numel() >= B * H * L
+    call("egovlp_text_attn_long_fwd", _ptr(qkv), _ptr(mask), _ptr(out), _ptr(lse), B, L, H, C.c_float(p_drop),
+         C.c_ulonglong(seed), C.c_uint(site), _stream())
+
+
+def text_attn_long_bwd(qkv, mask, out, lse, dout, dqkv, B, L, H, q_scale, p_drop=0.0, seed=0, site=0):
+    """Backward of text_attn_long_fwd (out / lse: its outputs) -> dqkv bf16 [B*L, 3*H*64]."""
+    assert mask.dtype == torch.int64 and mask.is_contiguous()
+    ws = torch.empty(B * H * L, dtype=F32, device=qkv.device)     # delta_i = rowsum(dO * O)
+    call("egovlp_text_attn_long_bwd", _ptr(qkv), _ptr(mask), _ptr(out), _ptr(lse), _ptr(dout), _ptr(dqkv), _ptr(ws),
+         B, L, H, C.c_float(q_scale), C.c_float(p_drop), C.c_ulonglong(seed), C.c_uint(site), _stream())
+
+
 def dropout(x, p, seed, site, add=None, y32=None, y16=None):
     """y = dropout_p(x) (+ add) with the (seed, site) Philox mask; returns (y32, y16) (whichever were given)."""
     _chk(x, F32, "x")

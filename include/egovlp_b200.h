@@ -170,8 +170,9 @@ int egovlp_video_embed_bwd(const float* dx, float* tmp_SD, float* dcls, float* d
 
 /* ------------------------------------------------------------------------------------------------
  * Text tower pieces (DistilBERT; call sites model/model.py:117-138).  ids / attention_mask are int64 as the
- * HuggingFace tokenizer returns them.  Head dim 64; L <= 128.
- *   text_embed_fwd : out fp32 [B*L, D] = word_emb[ids] + pos_emb[l]   (LayerNorm follows via egovlp_layernorm_fwd)
+ * HuggingFace tokenizer returns them.  Head dim 64; L <= 128 for text_attn_*, L <= 512 for text_attn_long_*.
+ *   text_embed_fwd : out fp32 [B*L, D] = word_emb[ids] + pos_emb[l]   (LayerNorm follows via egovlp_layernorm_fwd;
+ *                    the caller guarantees L <= rows of pos_emb)
  *   text_embed_bwd : dword[ids] += dsum, dpos[l] += dsum  (atomic accumulate)
  *   text_attn_fwd  : out bf16 [B*L, D] = softmax(q k^T + key-padding mask) v per (b, head); qkv bf16 [B*L, 3D],
  *                    q pre-scaled by 64^-0.5
@@ -180,6 +181,18 @@ int egovlp_video_embed_bwd(const float* dx, float* tmp_SD, float* dcls, float* d
  *                    in train mode (transformers modeling_distilbert.py, `weights = self.dropout(weights)`), mask
  *                    drawn from a counter-based Philox4x32-10 keyed by (seed, site) and indexed by (b, head, i, j);
  *                    the backward must be given the forward's (p_drop, seed, site).  p_drop = 0 disables it.
+ *   text_attn_long_fwd : the same attention for 1 <= L <= 512 (the text tower uses it above L = 128), tiled on the
+ *                    tensor cores (bf16 mma.sync, fp32 online softmax); 64-key tiles without a valid key are skipped.
+ *                    Also writes lse fp32 [B, H, L] (natural log of each row's softmax denominator, scores included),
+ *                    which the backward needs.  A sample whose mask is all zero gets NaN rows in out and lse.
+ *   text_attn_long_bwd : dqkv bf16 [B*L, 3D] (dq multiplied by q_scale; dk = dv = 0 for padded keys) from the
+ *                    forward's out and lse; workspace fp32 [B*H*L].  No floating-point atomics: bitwise reproducible.
+ *                    A sample whose mask is all zero gets dqkv = 0.
+ *                    Dropout as for text_attn, but the keep mask is its own stream: (b, h, i, j) is kept iff word
+ *                    (j & 3) of philox4x32_10(key(seed, site), ((b * 4096 + h) * 512 + i) * 128 + (j >> 2)) is
+ *                    >= p_drop * 2^32 (one Philox call per four keys; independent of B, H and L).
+ *                    Refused (EGOVLP_ERR_ARG, nothing written): a null pointer, L outside [1, 512], B outside
+ *                    [1, 65535], H outside [1, 4096], p_drop outside [0, 1).
  *   dropout        : y = dropout_p(x) (+ add), fp32 [n] -> fp32 y32 and / or bf16 y16 (n % 4 == 0).  The embedding and
  *                    FFN-output dropouts of DistilBERT (reference model/model.py:36 puts the text model in train mode);
  *                    calling it on a gradient with the same (p, seed, site) is the backward.
@@ -193,6 +206,11 @@ int egovlp_text_attn_fwd(const void* qkv, const long long* attention_mask, void*
                          unsigned long long seed, unsigned int site, void* stream);
 int egovlp_text_attn_bwd(const void* qkv, const long long* attention_mask, const void* dout, void* dqkv, int B, int L,
                          int H, float q_scale, float p_drop, unsigned long long seed, unsigned int site, void* stream);
+int egovlp_text_attn_long_fwd(const void* qkv, const long long* attention_mask, void* out, float* lse, int B, int L,
+                              int H, float p_drop, unsigned long long seed, unsigned int site, void* stream);
+int egovlp_text_attn_long_bwd(const void* qkv, const long long* attention_mask, const void* out, const float* lse,
+                              const void* dout, void* dqkv, float* workspace, int B, int L, int H, float q_scale,
+                              float p_drop, unsigned long long seed, unsigned int site, void* stream);
 int egovlp_dropout(const float* x, const float* add, float* y32, void* y16_bf16, long long n, float p,
                    unsigned long long seed, unsigned int site, void* stream);
 int egovlp_relu_rows_fwd(const float* x, long long row_stride, void* out_bf16, int rows, int D, void* stream);
