@@ -23,8 +23,8 @@ NVCC_FLAGS = ARCH + [ "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-I" + os.path.join(ROOT, "include"), "-I" + CSRC]
 # IEEE fp32 (no --use_fast_math: no approximate division / sqrt / exp, no flush-to-zero) where the reference computes in
 # fp32 and the results are compared at fp32 rounding level or bit-exactly: losses, ranking metrics, EgoMCQ, AdamW, and the
-# dataset video transforms (b / 255 and the normalisation are divisions, as torch's).
-IEEE_SOURCES = {"loss.cu", "loss_fused.cu", "retrieval.cu", "optim.cu", "video_transform.cu"}
+# dataset video transforms (b / 255 and the normalisation are divisions, as torch's), and the BERT pooler's tanh.
+IEEE_SOURCES = {"loss.cu", "loss_fused.cu", "retrieval.cu", "optim.cu", "video_transform.cu", "text_pooler.cu"}
 
 
 def flags_for(src):

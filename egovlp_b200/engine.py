@@ -93,6 +93,14 @@ class _CastEntry:
 _SHADOWS = {}          # id(param) -> _CastEntry: lets the fused AdamW write the bf16 copy in its own pass
 
 
+def _prune_shadows():
+    """Drop the entries of parameters that no longer exist, so that a dead model's bf16 copies are freed with it instead
+    of staying referenced here until the process ends (a process that builds several models in turn, such as the test
+    suite, would otherwise keep every one's copies on the device)."""
+    for key in [k for k, e in _SHADOWS.items() if e.ref() is None]:
+        del _SHADOWS[key]
+
+
 def shadow_entry(p):
     ent = _SHADOWS.get(id(p))
     return ent if ent is not None and ent.ref() is p and ent.t16.device == p.device else None
@@ -120,6 +128,7 @@ class Bf16Cache:
         if ent is None or ent.ref() is not p or ent.t16.device != p.device:
             ent = _CastEntry(p, t16_factory())
             self._store[id(p)] = ent
+            _prune_shadows()
             _SHADOWS[id(p)] = ent
             self._table = None
         if not ent.current(p):
@@ -606,11 +615,212 @@ class ClsHeadFn(torch.autograd.Function):
 
 
 # ----------------------------------------------------------------------------------------------------------
-# text tower (DistilBERT) + ReLU/Linear projection
+# text tower (DistilBERT / BERT) + ReLU/Linear projection
 # ----------------------------------------------------------------------------------------------------------
 # Longest caption the one-CTA-per-(sample, head) text attention (text_attn_*) takes; longer ones, up to the 512
 # positions of DistilBERT, run the tiled kernel (text_attn_long_*), which also keeps the rows' lse for the backward.
 TEXT_ATTN_SHORT_MAX_L = 128
+
+
+def _text_tower_fwd(ctx, bert, input_ids, attention_mask, heads, eps, tokens_mode, cache, drop, p):
+    """Forward of TextTowerFn (bert=False) and BertTowerFn (bert=True); see their docstrings for `p`."""
+    grad_mode = True
+    if isinstance(tokens_mode, tuple):
+        tokens_mode, grad_mode = tokens_mode
+    if bert:
+        word, pos, tt, elw, elb = p[:5]
+        qw_pool, qb_pool, pw, pb = p[-4:]
+        layer_p = p[5:-4]
+        tokens_mode = False          # the reference's compute_text_tokens returns the pooled output for BERT
+    else:
+        word, pos, elw, elb = p[:4]
+        pw, pb = p[-2:]
+        layer_p = p[4:-2]
+    layers = [layer_p[16 * i: 16 * (i + 1)] for i in range(len(layer_p) // 16)]
+    n_layers = len(layers)
+    B, L = input_ids.shape
+    if L > pos.shape[0]:
+        raise EgovlpError(f"text tower: sequence length {L} exceeds the {pos.shape[0]} position embeddings "
+                          "(max_position_embeddings); truncate the captions to that length")
+    D = word.shape[1]
+    M = B * L
+    long_attn = L > TEXT_ATTN_SHORT_MAX_L
+    ids = input_ids.contiguous().to(torch.int64)
+    mask = attention_mask.contiguous().to(torch.int64)
+    dev = word
+    train = grad_mode and any(ctx.needs_input_grad)
+    saved, lses = [], []
+    p_hid, p_att = (float(drop[0]), float(drop[1])) if drop else (0.0, 0.0)
+    seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if (p_hid > 0 or p_att > 0) else 0
+
+    emb = _empty((M, D), F32, dev)
+    # BERT: every token adds token-type row 0 (the reference passes no token_type_ids), folded into the positions
+    pos_tab = (pos.detach()[:L] + tt.detach()[0]) if bert else pos.detach()
+    ops.text_embed_fwd(ids, word.detach(), pos_tab, emb, B, L, D)
+    x, x16 = _empty((M, D), F32, dev), _empty((M, D), BF16, dev)
+    mean, rstd = _empty((M,), F32, dev), _empty((M,), F32, dev)
+    ops.layernorm_fwd(emb, elw.detach(), elb.detach(), eps, y16=x16, y32=x, mean=mean, rstd=rstd)
+    if p_hid > 0:
+        ops.dropout(x, p_hid, seed, 0, y32=x, y16=x16)                                # embeddings dropout (in place)
+    saved += [emb, mean, rstd]
+    for li, lp in enumerate(layers):
+        (qw, qb, kw, kb, vw, vb, ow, ob, sw, sb, l1w, l1b, l2w, l2b, fw, fb) = lp
+        wqkv = cache.cat(("text_qkv_w", li, id(qw)), (qw, kw, vw))
+        bqkv = torch.cat([qb.detach(), kb.detach(), vb.detach()])
+        HID = l1w.shape[0]
+        qkv = _empty((M, 3 * D), BF16, dev)
+        ops.gemm(x16, wqkv, qkv, bias=bqkv, col_scale=Q_SCALE, col_scale_ncols=D)
+        ctxv = _empty((M, D), BF16, dev)
+        if long_attn:
+            lse = _empty((B, heads, L), F32, dev)
+            ops.text_attn_long_fwd(qkv, mask, ctxv, lse, B, L, heads, p_att, seed, 1 + 2 * li)
+            lses.append(lse)
+        else:
+            ops.text_attn_fwd(qkv, mask, ctxv, B, L, heads, p_att, seed, 1 + 2 * li)
+        sa = _empty((M, D), F32, dev)
+        if bert and p_hid > 0:
+            ops.gemm(ctxv, cache.get(ow), sa, bias=ob.detach())
+            ops.dropout(sa, p_hid, seed, 1 + 2 * n_layers + li, add=x, y32=sa)          # BertSelfOutput: dropout + x
+        else:
+            ops.gemm(ctxv, cache.get(ow), sa, bias=ob.detach(), residual=x)           # sa_output + x
+        x1, x1_16 = _empty((M, D), F32, dev), _empty((M, D), BF16, dev)
+        m1, r1 = _empty((M,), F32, dev), _empty((M,), F32, dev)
+        ops.layernorm_fwd(sa, sw.detach(), sb.detach(), eps, y16=x1_16, y32=x1, mean=m1, rstd=r1)
+        hh, u = _empty((M, HID), BF16, dev), (_empty((M, HID), BF16, dev) if train else None)
+        ops.gemm(x1_16, cache.get(l1w), hh, bias=l1b.detach(), act=_ACT_FWD if train else 1, out2=u)
+        ff = _empty((M, D), F32, dev)
+        if p_hid > 0:
+            ops.gemm(hh, cache.get(l2w), ff, bias=l2b.detach())
+            ops.dropout(ff, p_hid, seed, 2 + 2 * li, add=x1, y32=ff)                   # dropout(ffn_output) + sa_output
+        else:
+            ops.gemm(hh, cache.get(l2w), ff, bias=l2b.detach(), residual=x1)          # ffn_output + sa_output
+        xn, xn16 = _empty((M, D), F32, dev), _empty((M, D), BF16, dev)
+        m2, r2 = _empty((M,), F32, dev), _empty((M,), F32, dev)
+        ops.layernorm_fwd(ff, fw.detach(), fb.detach(), eps, y16=xn16, y32=xn, mean=m2, rstd=r2)
+        saved += [x16, qkv, ctxv, sa, m1, r1, x1_16, u, hh, ff, m2, r2]
+        x, x16 = xn, xn16
+    rows, stride = (M, D) if tokens_mode else (B, L * D)
+    pooled = None
+    if bert:                       # pooler_output = tanh(dense(h_CLS)), and relu of it when txt_proj follows
+        pooled = _empty((B, D), F32, dev)
+        r16 = _empty((B, D), BF16, dev) if pw is not None else None
+        ops.text_pooler_fwd(x, L * D, qw_pool.detach(), qb_pool.detach(), pooled, r16, B, D)
+        out = pooled
+        if pw is not None:
+            out = _empty((B, pw.shape[0]), F32, dev)
+            _linear_fwd(r16, cache.get(pw), pb.detach(), out)
+    elif pw is None:               # projection='' (nn.Identity, model/model.py:80-82): the hidden state itself
+        r16 = None
+        out = x if tokens_mode else x.view(B, L * D)[:, :D].clone()
+    else:
+        r16 = _empty((rows, D), BF16, dev)
+        ops.relu_rows_fwd(x, stride, r16, rows, D)
+        out = _empty((rows, pw.shape[0]), F32, dev)
+        _linear_fwd(r16, cache.get(pw), pb.detach(), out)
+    if train:
+        ctx.meta = (B, L, D, heads, tokens_mode, n_layers, len(saved), p_hid, p_att, seed, bert)
+        ctx.cache = cache
+        ctx.has_proj = pw is not None
+        ctx.n_lse = len(lses)
+        ctx.save_for_backward(ids, mask, x, r16, pooled, *saved, *lses, *p[:len(p) - (0 if pw is not None else 2)])
+    return out.view(B, L, -1) if tokens_mode else out
+
+
+def _text_tower_bwd(ctx, dout):
+    B, L, D, heads, tokens_mode, n_layers, n_saved, p_hid, p_att, seed, bert = ctx.meta
+    cache = ctx.cache
+    sv = ctx.saved_tensors
+    ids, mask, x_last, r16, pooled = sv[:5]
+    saved = list(sv[5:5 + n_saved])
+    lses = sv[5 + n_saved:5 + n_saved + ctx.n_lse]          # one per layer when L > TEXT_ATTN_SHORT_MAX_L
+    p = sv[5 + n_saved + ctx.n_lse:]
+    head = 5 if bert else 4
+    if bert:
+        word, pos, tt, elw, elb = p[:5]
+    else:
+        word, pos, elw, elb = p[:4]
+    layers = [p[head + 16 * i: head + 16 * (i + 1)] for i in range(n_layers)]
+    M = B * L
+    rows, stride = (M, D) if tokens_mode else (B, L * D)
+    g_pw = g_pb = None
+    if ctx.has_proj:
+        pw, pb = p[-2:]
+        Pd = pw.shape[0]
+        dout = dout.contiguous().float().view(rows, Pd)
+        g_pw, g_pb, dr = _linear_bwd(dout, r16, cache.get(pw))
+    if bert:
+        qw_pool = p[head + 16 * n_layers]
+        g_in = dr if ctx.has_proj else dout.contiguous().float().view(B, D)
+        dx = _zeros((M, D), g_in)
+        g_qw_pool, g_qb_pool = _empty((D, D), F32, g_in), _empty((D,), F32, g_in)
+        ops.text_pooler_bwd(g_in, pooled, ctx.has_proj, x_last, L * D, qw_pool.detach(), g_qw_pool, g_qb_pool, dx, B, D)
+        dout = g_in
+    elif ctx.has_proj:
+        dx = _zeros((M, D), dout)
+        ops.relu_rows_bwd(x_last, stride, dr, dx, rows, D)
+    else:
+        dout = dout.contiguous().float().view(rows, D)
+        if tokens_mode:
+            dx = dout
+        else:
+            dx = _zeros((M, D), dout)
+            dx.view(B, L * D)[:, :D].copy_(dout)
+    grads = []
+    for li in reversed(range(n_layers)):
+        (qw, qb, kw, kb, vw, vb, ow, ob, sw, sb, l1w, l1b, l2w, l2b, fw, fb) = layers[li]
+        x16, qkv, ctxv, sa, m1, r1, x1_16, u, hh, ff, m2, r2 = saved[3 + 12 * li: 3 + 12 * (li + 1)]
+        HID = l1w.shape[0]
+        dff, dff16 = _empty((M, D), F32, dout), _empty((M, D), BF16, dout)
+        g_fw, g_fb = _zeros((D,), dout), _zeros((D,), dout)
+        ops.layernorm_bwd(dx, ff, fw.detach(), m2, r2, dx=dff, dx16=dff16, dgamma=g_fw, dbeta=g_fb)
+        dffn, dffn16 = dff, dff16                      # gradient of the FFN output (before its dropout)
+        if p_hid > 0:
+            dffn, dffn16 = _empty((M, D), F32, dout), _empty((M, D), BF16, dout)
+            ops.dropout(dff, p_hid, seed, 2 + 2 * li, y32=dffn, y16=dffn16)
+        g_l2w, g_l2b = wgrad(dffn16, hh, D, HID), bgrad(dffn)
+        du = _empty((M, HID), BF16, dout)
+        ops.gemm(dffn16, cache.get(l2w), du, b_mn=True, aux=u, act=_ACT_BWD)
+        g_l1w, g_l1b = wgrad(du, x1_16, HID, D), bgrad(du)
+        dx1 = _empty((M, D), F32, dout)
+        ops.gemm(du, cache.get(l1w), dx1, b_mn=True, residual=dff)                     # + residual path
+        dsa, dsa16 = _empty((M, D), F32, dout), _empty((M, D), BF16, dout)
+        g_sw, g_sb = _zeros((D,), dout), _zeros((D,), dout)
+        ops.layernorm_bwd(dx1, sa, sw.detach(), m1, r1, dx=dsa, dx16=dsa16, dgamma=g_sw, dbeta=g_sb)
+        dso, dso16 = dsa, dsa16                        # gradient of the attention output dense (before its dropout)
+        if bert and p_hid > 0:
+            dso, dso16 = _empty((M, D), F32, dout), _empty((M, D), BF16, dout)
+            ops.dropout(dsa, p_hid, seed, 1 + 2 * n_layers + li, y32=dso, y16=dso16)
+        g_ow, g_ob = wgrad(dso16, ctxv, D, D), bgrad(dso)
+        dctx = _empty((M, D), BF16, dout)
+        ops.gemm(dso16, cache.get(ow), dctx, b_mn=True)
+        dqkv = _empty((M, 3 * D), BF16, dout)
+        if lses:
+            ops.text_attn_long_bwd(qkv, mask, ctxv, lses[li], dctx, dqkv, B, L, heads, Q_SCALE, p_att, seed,
+                                   1 + 2 * li)
+        else:
+            ops.text_attn_bwd(qkv, mask, dctx, dqkv, B, L, heads, Q_SCALE, p_att, seed, 1 + 2 * li)
+        g_wqkv, g_bqkv = wgrad(dqkv, x16, 3 * D, D), bgrad(dqkv)
+        wqkv = cache.cat(("text_qkv_w", li, id(qw)), (qw, kw, vw))
+        dxin = _empty((M, D), F32, dout)
+        ops.gemm(dqkv, wqkv, dxin, b_mn=True, residual=dsa)                            # x feeds qkv and the residual
+        dx = dxin
+        gq, gk, gv = g_wqkv[:D], g_wqkv[D:2 * D], g_wqkv[2 * D:]
+        bq, bk, bv = g_bqkv[:D], g_bqkv[D:2 * D], g_bqkv[2 * D:]
+        grads = [gq, bq, gk, bk, gv, bv, g_ow, g_ob, g_sw, g_sb, g_l1w, g_l1b, g_l2w, g_l2b, g_fw, g_fb] + grads
+    emb, mean, rstd = saved[:3]
+    if p_hid > 0:
+        ops.dropout(dx, p_hid, seed, 0, y32=dx)                                       # embeddings dropout, backward
+    demb = _empty((M, D), F32, dout)
+    g_elw, g_elb = _zeros((D,), dout), _zeros((D,), dout)
+    ops.layernorm_bwd(dx, emb, elw.detach(), mean, rstd, dx=demb, dgamma=g_elw, dbeta=g_elb)
+    g_word, g_pos = torch.zeros_like(word), torch.zeros_like(pos)
+    ops.text_embed_bwd(ids, demb, g_word, g_pos, B, L, D)
+    if not bert:
+        return (None, None, None, None, None, None, None, g_word, g_pos, g_elw, g_elb, *grads, g_pw, g_pb)
+    g_tt = torch.zeros_like(tt)
+    g_tt[0] = g_pos[:L].sum(0)                         # token-type row 0 was added to every position row
+    return (None, None, None, None, None, None, None, g_word, g_pos, g_tt, g_elw, g_elb, *grads, g_qw_pool, g_qb_pool,
+            g_pw, g_pb)
 
 
 class TextTowerFn(torch.autograd.Function):
@@ -623,164 +833,41 @@ class TextTowerFn(torch.autograd.Function):
     on the attention probabilities and on the FFN output (modeling_distilbert.py; the reference calls
     `self.text_model.train()`, model/model.py:36).  Masks come from a counter-based Philox stream keyed by one seed
     drawn per forward from torch's CPU generator (so `torch.manual_seed` makes a run reproducible); the backward
-    regenerates them.  (0, 0) = eval mode / the deterministic parity path."""
+    regenerates them.  Philox sites: 0 = embeddings, 1 + 2 * layer = attention probabilities, 2 + 2 * layer = FFN
+    output.  (0, 0) = eval mode / the deterministic parity path."""
 
     @staticmethod
     def forward(ctx, input_ids, attention_mask, heads, eps, tokens_mode, cache, drop, *p):
         """`tokens_mode`: False / True, or a (tokens_mode, grad_mode) pair -- see SpaceTimeBlockFn.forward."""
-        grad_mode = True
-        if isinstance(tokens_mode, tuple):
-            tokens_mode, grad_mode = tokens_mode
-        word, pos, elw, elb = p[:4]
-        pw, pb = p[-2:]
-        layers = [p[4 + 16 * i: 4 + 16 * (i + 1)] for i in range((len(p) - 6) // 16)]
-        B, L = input_ids.shape
-        if L > pos.shape[0]:
-            raise EgovlpError(f"text tower: sequence length {L} exceeds the {pos.shape[0]} position embeddings "
-                              "(max_position_embeddings); truncate the captions to that length")
-        D = word.shape[1]
-        M = B * L
-        long_attn = L > TEXT_ATTN_SHORT_MAX_L
-        ids = input_ids.contiguous().to(torch.int64)
-        mask = attention_mask.contiguous().to(torch.int64)
-        dev = word
-        train = grad_mode and any(ctx.needs_input_grad)
-        saved, lses = [], []
-        p_hid, p_att = (float(drop[0]), float(drop[1])) if drop else (0.0, 0.0)
-        seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if (p_hid > 0 or p_att > 0) else 0
-
-        emb = _empty((M, D), F32, dev)
-        ops.text_embed_fwd(ids, word.detach(), pos.detach(), emb, B, L, D)
-        x, x16 = _empty((M, D), F32, dev), _empty((M, D), BF16, dev)
-        mean, rstd = _empty((M,), F32, dev), _empty((M,), F32, dev)
-        ops.layernorm_fwd(emb, elw.detach(), elb.detach(), eps, y16=x16, y32=x, mean=mean, rstd=rstd)
-        if p_hid > 0:
-            ops.dropout(x, p_hid, seed, 0, y32=x, y16=x16)                                # embeddings dropout (in place)
-        saved += [emb, mean, rstd]
-        for li, lp in enumerate(layers):
-            (qw, qb, kw, kb, vw, vb, ow, ob, sw, sb, l1w, l1b, l2w, l2b, fw, fb) = lp
-            wqkv = cache.cat(("text_qkv_w", li, id(qw)), (qw, kw, vw))
-            bqkv = torch.cat([qb.detach(), kb.detach(), vb.detach()])
-            HID = l1w.shape[0]
-            qkv = _empty((M, 3 * D), BF16, dev)
-            ops.gemm(x16, wqkv, qkv, bias=bqkv, col_scale=Q_SCALE, col_scale_ncols=D)
-            ctxv = _empty((M, D), BF16, dev)
-            if long_attn:
-                lse = _empty((B, heads, L), F32, dev)
-                ops.text_attn_long_fwd(qkv, mask, ctxv, lse, B, L, heads, p_att, seed, 1 + 2 * li)
-                lses.append(lse)
-            else:
-                ops.text_attn_fwd(qkv, mask, ctxv, B, L, heads, p_att, seed, 1 + 2 * li)
-            sa = _empty((M, D), F32, dev)
-            ops.gemm(ctxv, cache.get(ow), sa, bias=ob.detach(), residual=x)               # sa_output + x
-            x1, x1_16 = _empty((M, D), F32, dev), _empty((M, D), BF16, dev)
-            m1, r1 = _empty((M,), F32, dev), _empty((M,), F32, dev)
-            ops.layernorm_fwd(sa, sw.detach(), sb.detach(), eps, y16=x1_16, y32=x1, mean=m1, rstd=r1)
-            hh, u = _empty((M, HID), BF16, dev), (_empty((M, HID), BF16, dev) if train else None)
-            ops.gemm(x1_16, cache.get(l1w), hh, bias=l1b.detach(), act=_ACT_FWD if train else 1, out2=u)
-            ff = _empty((M, D), F32, dev)
-            if p_hid > 0:
-                ops.gemm(hh, cache.get(l2w), ff, bias=l2b.detach())
-                ops.dropout(ff, p_hid, seed, 2 + 2 * li, add=x1, y32=ff)                   # dropout(ffn_output) + sa_output
-            else:
-                ops.gemm(hh, cache.get(l2w), ff, bias=l2b.detach(), residual=x1)          # ffn_output + sa_output
-            xn, xn16 = _empty((M, D), F32, dev), _empty((M, D), BF16, dev)
-            m2, r2 = _empty((M,), F32, dev), _empty((M,), F32, dev)
-            ops.layernorm_fwd(ff, fw.detach(), fb.detach(), eps, y16=xn16, y32=xn, mean=m2, rstd=r2)
-            saved += [x16, qkv, ctxv, sa, m1, r1, x1_16, u, hh, ff, m2, r2]
-            x, x16 = xn, xn16
-        rows, stride = (M, D) if tokens_mode else (B, L * D)
-        if pw is None:                 # projection='' (nn.Identity, model/model.py:80-82): the hidden state itself
-            r16 = None
-            out = x if tokens_mode else x.view(B, L * D)[:, :D].clone()
-        else:
-            r16 = _empty((rows, D), BF16, dev)
-            ops.relu_rows_fwd(x, stride, r16, rows, D)
-            out = _empty((rows, pw.shape[0]), F32, dev)
-            _linear_fwd(r16, cache.get(pw), pb.detach(), out)
-        if train:
-            ctx.meta = (B, L, D, heads, tokens_mode, len(layers), len(saved), p_hid, p_att, seed)
-            ctx.cache = cache
-            ctx.has_proj = pw is not None
-            ctx.n_lse = len(lses)
-            ctx.save_for_backward(ids, mask, x, r16, *saved, *lses, *p[:len(p) - (0 if pw is not None else 2)])
-        return out.view(B, L, -1) if tokens_mode else out
+        return _text_tower_fwd(ctx, False, input_ids, attention_mask, heads, eps, tokens_mode, cache, drop, p)
 
     @staticmethod
     def backward(ctx, dout):
-        B, L, D, heads, tokens_mode, n_layers, n_saved, p_hid, p_att, seed = ctx.meta
-        cache = ctx.cache
-        sv = ctx.saved_tensors
-        ids, mask, x_last, r16 = sv[:4]
-        saved = list(sv[4:4 + n_saved])
-        lses = sv[4 + n_saved:4 + n_saved + ctx.n_lse]          # one per layer when L > TEXT_ATTN_SHORT_MAX_L
-        p = sv[4 + n_saved + ctx.n_lse:]
-        word, pos, elw, elb = p[:4]
-        layers = [p[4 + 16 * i: 4 + 16 * (i + 1)] for i in range(n_layers)]
-        M = B * L
-        rows, stride = (M, D) if tokens_mode else (B, L * D)
-        if ctx.has_proj:
-            pw, pb = p[-2:]
-            Pd = pw.shape[0]
-            dout = dout.contiguous().float().view(rows, Pd)
-            g_pw, g_pb, dr = _linear_bwd(dout, r16, cache.get(pw))
-            dx = _zeros((M, D), dout)
-            ops.relu_rows_bwd(x_last, stride, dr, dx, rows, D)
-        else:
-            g_pw = g_pb = None
-            dout = dout.contiguous().float().view(rows, D)
-            if tokens_mode:
-                dx = dout
-            else:
-                dx = _zeros((M, D), dout)
-                dx.view(B, L * D)[:, :D].copy_(dout)
-        grads = []
-        for li in reversed(range(n_layers)):
-            (qw, qb, kw, kb, vw, vb, ow, ob, sw, sb, l1w, l1b, l2w, l2b, fw, fb) = layers[li]
-            x16, qkv, ctxv, sa, m1, r1, x1_16, u, hh, ff, m2, r2 = saved[3 + 12 * li: 3 + 12 * (li + 1)]
-            HID = l1w.shape[0]
-            dff, dff16 = _empty((M, D), F32, dout), _empty((M, D), BF16, dout)
-            g_fw, g_fb = _zeros((D,), dout), _zeros((D,), dout)
-            ops.layernorm_bwd(dx, ff, fw.detach(), m2, r2, dx=dff, dx16=dff16, dgamma=g_fw, dbeta=g_fb)
-            dffn, dffn16 = dff, dff16                      # gradient of the FFN output (before its dropout)
-            if p_hid > 0:
-                dffn, dffn16 = _empty((M, D), F32, dout), _empty((M, D), BF16, dout)
-                ops.dropout(dff, p_hid, seed, 2 + 2 * li, y32=dffn, y16=dffn16)
-            g_l2w, g_l2b = wgrad(dffn16, hh, D, HID), bgrad(dffn)
-            du = _empty((M, HID), BF16, dout)
-            ops.gemm(dffn16, cache.get(l2w), du, b_mn=True, aux=u, act=_ACT_BWD)
-            g_l1w, g_l1b = wgrad(du, x1_16, HID, D), bgrad(du)
-            dx1 = _empty((M, D), F32, dout)
-            ops.gemm(du, cache.get(l1w), dx1, b_mn=True, residual=dff)                     # + residual path
-            dsa, dsa16 = _empty((M, D), F32, dout), _empty((M, D), BF16, dout)
-            g_sw, g_sb = _zeros((D,), dout), _zeros((D,), dout)
-            ops.layernorm_bwd(dx1, sa, sw.detach(), m1, r1, dx=dsa, dx16=dsa16, dgamma=g_sw, dbeta=g_sb)
-            g_ow, g_ob = wgrad(dsa16, ctxv, D, D), bgrad(dsa)
-            dctx = _empty((M, D), BF16, dout)
-            ops.gemm(dsa16, cache.get(ow), dctx, b_mn=True)
-            dqkv = _empty((M, 3 * D), BF16, dout)
-            if lses:
-                ops.text_attn_long_bwd(qkv, mask, ctxv, lses[li], dctx, dqkv, B, L, heads, Q_SCALE, p_att, seed,
-                                       1 + 2 * li)
-            else:
-                ops.text_attn_bwd(qkv, mask, dctx, dqkv, B, L, heads, Q_SCALE, p_att, seed, 1 + 2 * li)
-            g_wqkv, g_bqkv = wgrad(dqkv, x16, 3 * D, D), bgrad(dqkv)
-            wqkv = cache.cat(("text_qkv_w", li, id(qw)), (qw, kw, vw))
-            dxin = _empty((M, D), F32, dout)
-            ops.gemm(dqkv, wqkv, dxin, b_mn=True, residual=dsa)                            # x feeds qkv and the residual
-            dx = dxin
-            gq, gk, gv = g_wqkv[:D], g_wqkv[D:2 * D], g_wqkv[2 * D:]
-            bq, bk, bv = g_bqkv[:D], g_bqkv[D:2 * D], g_bqkv[2 * D:]
-            grads = [gq, bq, gk, bk, gv, bv, g_ow, g_ob, g_sw, g_sb, g_l1w, g_l1b, g_l2w, g_l2b, g_fw, g_fb] + grads
-        emb, mean, rstd = saved[:3]
-        if p_hid > 0:
-            ops.dropout(dx, p_hid, seed, 0, y32=dx)                                       # embeddings dropout, backward
-        demb = _empty((M, D), F32, dout)
-        g_elw, g_elb = _zeros((D,), dout), _zeros((D,), dout)
-        ops.layernorm_bwd(dx, emb, elw.detach(), mean, rstd, dx=demb, dgamma=g_elw, dbeta=g_elb)
-        g_word, g_pos = torch.zeros_like(word), torch.zeros_like(pos)
-        ops.text_embed_bwd(ids, demb, g_word, g_pos, B, L, D)
-        return (None, None, None, None, None, None, None, g_word, g_pos, g_elw, g_elb, *grads, g_pw, g_pb)
+        return _text_tower_bwd(ctx, dout)
+
+
+class BertTowerFn(torch.autograd.Function):
+    """BertModel(input_ids, attention_mask=...)['pooler_output'] -> ReLU -> Linear  (model/model.py:117-138, the
+    `bert*` branch).  The encoder layers run exactly as TextTowerFn's; BERT adds token-type row 0 to every embedding
+    (the reference passes no token_type_ids), a dropout on the attention output dense, and the pooler
+    tanh(dense(h_CLS)) in place of the CLS row.  tokens_mode gives the pooled result too, as the reference's
+    compute_text_tokens does for BERT.
+
+    params: word_emb, pos_emb, token_type_emb, emb_ln.{w,b}, then per layer
+            query.{w,b}, key.{w,b}, value.{w,b}, attention.output.dense.{w,b}, attention.output.LayerNorm.{w,b},
+            intermediate.dense.{w,b}, output.dense.{w,b}, output.LayerNorm.{w,b}   (16 / layer),
+            then pooler.dense.{w,b}, finally txt_proj.{w,b} (None, None for projection='').
+    `drop` = (hidden_dropout_prob, attention_probs_dropout_prob), applied as HF BERT does in train mode.  Philox sites
+    (n = number of layers): 0 = embeddings, 1 + 2 * layer = attention probabilities, 2 + 2 * layer = FFN output,
+    1 + 2 * n + layer = attention output dense."""
+
+    @staticmethod
+    def forward(ctx, input_ids, attention_mask, heads, eps, tokens_mode, cache, drop, *p):
+        return _text_tower_fwd(ctx, True, input_ids, attention_mask, heads, eps, tokens_mode, cache, drop, p)
+
+    @staticmethod
+    def backward(ctx, dout):
+        return _text_tower_bwd(ctx, dout)
 
 
 # ----------------------------------------------------------------------------------------------------------

@@ -51,6 +51,52 @@ def _build_distilbert(text_params):
         return DistilBertModel(DistilBertConfig())
 
 
+# Architectures a `bert*` name random-initialises to when its files are not present:
+# (hidden_size, num_hidden_layers, num_attention_heads, intermediate_size, vocab_size)
+_BERT_ARCHS = {'bert-base-uncased': (768, 12, 12, 3072, 30522), 'bert-base-cased': (768, 12, 12, 3072, 28996),
+               'bert-large-uncased': (1024, 24, 16, 4096, 30522), 'bert-large-cased': (1024, 24, 16, 4096, 28996)}
+
+
+def _build_bert(name):
+    """Parameter container for a `bert*` text tower (reference model/model.py:34-35): the HuggingFace BertModel of
+    `name` (weights only; its forward is not used).  Loads the local files when present, otherwise random-initialises
+    the named architecture; any other name without files raises."""
+    from transformers import AutoModel, BertConfig, BertModel
+    try:
+        return AutoModel.from_pretrained(name, local_files_only=True)
+    except Exception:  # no network / no files: synthetic-weights path
+        if name not in _BERT_ARCHS:
+            raise NotImplementedError(f"{name}: no local files, and not one of {sorted(_BERT_ARCHS)} whose "
+                                      "architecture can be random-initialised without them")
+        warnings.warn(f"{name} files not found: text tower is randomly initialised")
+        hid, layers, heads, inter, vocab = _BERT_ARCHS[name]
+        return BertModel(BertConfig(hidden_size=hid, num_hidden_layers=layers, num_attention_heads=heads,
+                                    intermediate_size=inter, vocab_size=vocab))
+
+
+def _check_bert(tm):
+    """Refuse, naming the field, a BERT the CUDA tower does not run: it takes the post-LN encoder with absolute
+    positions, exact GELU, head dim 64, hidden <= 1024 and the pooler."""
+    from transformers import BertModel
+    if not isinstance(tm, BertModel):
+        raise NotImplementedError(f"text model {type(tm).__name__}: only BertModel runs as a `bert*` text tower")
+    cfg = tm.config
+    if cfg.hidden_size % cfg.num_attention_heads or cfg.hidden_size // cfg.num_attention_heads != 64:
+        raise NotImplementedError(f"num_attention_heads={cfg.num_attention_heads}: the text tower needs head dim 64 "
+                                  f"(hidden_size={cfg.hidden_size})")
+    if cfg.hidden_size > 1024:
+        raise NotImplementedError(f"hidden_size={cfg.hidden_size}: the text tower takes hidden_size <= 1024")
+    if cfg.hidden_act != 'gelu':
+        raise NotImplementedError(f"hidden_act={cfg.hidden_act!r}: the text tower implements 'gelu' (exact erf)")
+    if getattr(cfg, 'position_embedding_type', 'absolute') != 'absolute':
+        raise NotImplementedError(f"position_embedding_type={cfg.position_embedding_type!r}: the text tower "
+                                  "implements 'absolute'")
+    if cfg.is_decoder or getattr(cfg, 'add_cross_attention', False):
+        raise NotImplementedError("is_decoder / add_cross_attention: the text tower is an encoder")
+    if tm.pooler is None:
+        raise NotImplementedError("pooler: a BertModel built with add_pooling_layer=False has no pooler_output")
+
+
 _VIT_B16_FILE = "pretrained/jx_vit_base_p16_224-80ecf9dd.pth"
 
 
@@ -86,9 +132,16 @@ class FrozenInTime(BaseModel):
         self.video_params, self.text_params, self.load_temporal_fix = video_params, text_params, load_temporal_fix
         if not text_params['pretrained']:
             raise NotImplementedError("Huggingface text models require pretrained init.")
-        if not text_params['model'].startswith('distilbert'):
-            raise NotImplementedError(f"{text_params['model']}: only the DistilBERT text tower is implemented")
-        self.text_model = _build_distilbert(text_params)
+        name = text_params['model']
+        self._bert = name.startswith('bert')
+        if self._bert:
+            self.text_model = _build_bert(name)
+            _check_bert(self.text_model)
+        elif name.startswith('distilbert'):
+            self.text_model = _build_distilbert(text_params)
+        else:
+            raise NotImplementedError(f"{name}: the text tower implements DistilBERT (`distilbert*`) and BERT "
+                                      "(`bert*`)")
         self.text_model.train()                                   # as the reference: HF dropouts active while training
         restoring = load_checkpoint not in ("", None)
         self.video_model = _build_video_tower(video_params, from_scratch=not restoring)
@@ -130,6 +183,18 @@ class FrozenInTime(BaseModel):
     # ---- text ------------------------------------------------------------------------------------------------
     def _text_params(self):
         tm = self.text_model
+        if self._bert:
+            e = tm.embeddings
+            p = [e.word_embeddings.weight, e.position_embeddings.weight, e.token_type_embeddings.weight,
+                 e.LayerNorm.weight, e.LayerNorm.bias]
+            for layer in tm.encoder.layer:
+                a = layer.attention
+                for lin in (a.self.query, a.self.key, a.self.value, a.output.dense):
+                    p += [lin.weight, lin.bias]
+                p += [a.output.LayerNorm.weight, a.output.LayerNorm.bias, layer.intermediate.dense.weight,
+                      layer.intermediate.dense.bias, layer.output.dense.weight, layer.output.dense.bias,
+                      layer.output.LayerNorm.weight, layer.output.LayerNorm.bias]
+            return p + [tm.pooler.dense.weight, tm.pooler.dense.bias]
         p = [tm.embeddings.word_embeddings.weight, tm.embeddings.position_embeddings.weight,
              tm.embeddings.LayerNorm.weight, tm.embeddings.LayerNorm.bias]
         for layer in tm.transformer.layer:
@@ -141,13 +206,24 @@ class FrozenInTime(BaseModel):
         return p
 
     def _text(self, text_data, tokens_mode, _refresh=True):
-        # projection='' (nn.Identity, reference :80-82): the tower ends at the DistilBERT hidden state (no ReLU / Linear)
+        # projection='' (nn.Identity, reference :80-82): the tower ends at the DistilBERT hidden state / the BERT pooler
+        # output (no ReLU / Linear)
         proj = self.txt_proj[1] if isinstance(self.txt_proj, nn.Sequential) else None
         cfg = self.text_model.config
         if _refresh and torch.is_grad_enabled():
             self._bf16_cache.refresh()
         # train-mode dropouts of the HF text model (the reference keeps `text_model.train()`, :36); eval() or a config
         # with dropout = attention_dropout = 0 gives the deterministic path
+        # (BERT: input_ids and attention_mask only -- the reference passes no token_type_ids, so every token gets
+        # token type 0, and its compute_text_tokens returns the pooled output as compute_text does, :129-131)
+        if self._bert:
+            drop = ((cfg.hidden_dropout_prob, cfg.attention_probs_dropout_prob) if self.text_model.training
+                    else (0.0, 0.0))
+            return engine.BertTowerFn.apply(text_data['input_ids'], text_data['attention_mask'],
+                                            cfg.num_attention_heads, cfg.layer_norm_eps,
+                                            (False, torch.is_grad_enabled()), self._bf16_cache, drop,
+                                            *self._text_params(),
+                                            *((proj.weight, proj.bias) if proj is not None else (None, None)))
         drop = (cfg.dropout, cfg.attention_dropout) if self.text_model.training else (0.0, 0.0)
         return engine.TextTowerFn.apply(text_data['input_ids'], text_data['attention_mask'], cfg.n_heads, 1e-12,
                                         (tokens_mode, torch.is_grad_enabled()), self._bf16_cache, drop, *self._text_params(),

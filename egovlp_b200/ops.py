@@ -398,6 +398,24 @@ def relu_rows_bwd(x, row_stride, dh, dx, rows, D):
     call("egovlp_relu_rows_bwd", _ptr(x), C.c_longlong(row_stride), _ptr(dh), _ptr(dx), rows, D, _stream())
 
 
+def text_pooler_fwd(h, row_stride, w, b, y, relu16, B, D):
+    """BERT pooler: y fp32 [B, D] = tanh(W h_CLS + b) from the CLS rows h[r * row_stride + :D]; relu16 (bf16 [B, D] or
+    None) = relu(y)."""
+    _chk(h, F32, "h"); _chk(w, F32, "w"); _chk(b, F32, "b"); _chk(y, F32, "y")
+    if relu16 is not None:
+        _chk(relu16, BF16, "relu16")
+    call("egovlp_text_pooler_fwd", _ptr(h), C.c_longlong(row_stride), _ptr(w), _ptr(b), _ptr(y), _ptr(relu16), B, D,
+         _stream())
+
+
+def text_pooler_bwd(g, y, relu, h, row_stride, w, dw, db, dh, B, D):
+    """Backward of text_pooler_fwd from the gradient at relu(y) (relu=True) or at y: writes dw, db and the CLS rows of dh."""
+    for t, name in ((g, "g"), (y, "y"), (h, "h"), (w, "w"), (dw, "dw"), (db, "db"), (dh, "dh")):
+        _chk(t, F32, name)
+    call("egovlp_text_pooler_bwd", _ptr(g), _ptr(y), int(bool(relu)), _ptr(h), C.c_longlong(row_stride), _ptr(w),
+         _ptr(dw), _ptr(db), _ptr(dh), B, D, _stream())
+
+
 # ---------------------------------------------------------------- narrow projection heads (C % 32 != 0)
 def narrow_linear_fwd(act16, w16, bias, out):
     """out fp32 [rows, C] = act16 [rows, K] @ w16 [C, K]^T + bias (fp32 [C])."""

@@ -16,10 +16,14 @@ IMAGENET_STD = (0.229, 0.224, 0.225)
 
 def model_dims(embed_dim=768, depth=12, heads=12, mlp_ratio=4, patch=16, img=224, num_frames=16,
                text_dim=768, text_layers=6, text_heads=12, text_hidden=3072, vocab=30522, max_pos=512,
-               proj_dim=256):
-    return dict(embed_dim=embed_dim, depth=depth, heads=heads, mlp_hidden=int(embed_dim * mlp_ratio), patch=patch,
+               proj_dim=256, text_kind=None):
+    """`text_kind='bert'`: a BERT text tower (token-type table, BERT key names, pooler); None = DistilBERT."""
+    dims = dict(embed_dim=embed_dim, depth=depth, heads=heads, mlp_hidden=int(embed_dim * mlp_ratio), patch=patch,
                 img=img, num_frames=num_frames, text_dim=text_dim, text_layers=text_layers, text_heads=text_heads,
                 text_hidden=text_hidden, vocab=vocab, max_pos=max_pos, proj_dim=proj_dim)
+    if text_kind is not None:
+        dims["text_kind"] = text_kind
+    return dims
 
 
 # small geometry used by the tests: head_dim stays 64 (the attention kernels are specialised for it)
@@ -27,12 +31,39 @@ TINY_DIMS = model_dims(embed_dim=128, depth=2, heads=2, patch=16, img=32, num_fr
                        text_heads=2, text_hidden=256, vocab=120, max_pos=32, proj_dim=32)
 
 
+def _bert_shapes(dims, s):
+    """transformers BertModel keys (token types 2, pooler) under text_model., in its registration order."""
+    E, TH = dims["text_dim"], dims["text_hidden"]
+    s["text_model.embeddings.word_embeddings.weight"] = (dims["vocab"], E)
+    s["text_model.embeddings.position_embeddings.weight"] = (dims["max_pos"], E)
+    s["text_model.embeddings.token_type_embeddings.weight"] = (2, E)
+    s["text_model.embeddings.LayerNorm.weight"] = (E,)
+    s["text_model.embeddings.LayerNorm.bias"] = (E,)
+    for i in range(dims["text_layers"]):
+        lp = f"text_model.encoder.layer.{i}."
+        for lin in ("self.query", "self.key", "self.value", "output.dense"):
+            s[lp + f"attention.{lin}.weight"] = (E, E)
+            s[lp + f"attention.{lin}.bias"] = (E,)
+        s[lp + "attention.output.LayerNorm.weight"] = (E,)
+        s[lp + "attention.output.LayerNorm.bias"] = (E,)
+        s[lp + "intermediate.dense.weight"] = (TH, E)
+        s[lp + "intermediate.dense.bias"] = (TH,)
+        s[lp + "output.dense.weight"] = (E, TH)
+        s[lp + "output.dense.bias"] = (E,)
+        s[lp + "output.LayerNorm.weight"] = (E,)
+        s[lp + "output.LayerNorm.bias"] = (E,)
+    s["text_model.pooler.dense.weight"] = (E, E)
+    s["text_model.pooler.dense.bias"] = (E,)
+
+
 def state_dict_shapes(dims, video=True, text=True, proj=True):
     """Ordered {key: shape} in the reference's registration order."""
     D, H, P = dims["embed_dim"], dims["mlp_hidden"], dims["patch"]
     n = (dims["img"] // P) ** 2
     s = OrderedDict()
-    if text:
+    if text and dims.get("text_kind") == "bert":
+        _bert_shapes(dims, s)
+    elif text:
         E, TH = dims["text_dim"], dims["text_hidden"]
         s["text_model.embeddings.word_embeddings.weight"] = (dims["vocab"], E)
         s["text_model.embeddings.position_embeddings.weight"] = (dims["max_pos"], E)
@@ -96,7 +127,7 @@ def seeded_state_dict(dims, seed=0, video=True, text=True, proj=True, dtype=torc
             t = 1.0 + 0.1 * r
         elif k.endswith(".bias"):
             t = 0.02 * r
-        elif "word_embeddings" in k or "position_embeddings" in k:
+        elif "word_embeddings" in k or "position_embeddings" in k or "token_type_embeddings" in k:
             t = 0.05 * r
         elif k.endswith(("cls_token", "pos_embed", "temporal_embed")):
             t = 0.02 * r

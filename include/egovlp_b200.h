@@ -217,6 +217,23 @@ int egovlp_relu_rows_fwd(const float* x, long long row_stride, void* out_bf16, i
 int egovlp_relu_rows_bwd(const float* x, long long row_stride, const float* dh, float* dx, int rows, int D, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * BERT pooler (transformers modeling_bert.py BertPooler), the text embedding of the reference's `bert*` tower:
+ * `self.text_model(...)['pooler_output']` (model/model.py:117-131), followed by txt_proj's ReLU (model/model.py:73-75).
+ * fp32, no atomics (bitwise reproducible).  1 <= B, 4 <= D <= 1024, D % 4 == 0, row_stride >= D; otherwise
+ * EGOVLP_ERR_ARG and nothing is launched.
+ *   text_pooler_fwd : y fp32 [B, D] = tanh(h[b * row_stride + :D] W^T + bias), W fp32 [D, D] (nn.Linear layout);
+ *                     h = the CLS rows read in place from the [B*L, D] hidden state (row_stride = L * D).
+ *                     relu_bf16 (optional, bf16 [B, D]) = relu(y): the txt_proj GEMM operand.
+ *   text_pooler_bwd : from grad fp32 [B, D] at relu(y) (relu != 0) or at y (relu == 0, projection=''):
+ *                     dz = grad * [y > 0 if relu] * (1 - y^2); writes dweight fp32 [D, D] = dz^T h, dbias [D] = sum_b dz,
+ *                     dh[b * row_stride + :D] = dz W (only the B CLS rows of dh are written).
+ */
+int egovlp_text_pooler_fwd(const float* h, long long row_stride, const float* weight, const float* bias, float* y,
+                           void* relu_bf16, int B, int D, void* stream);
+int egovlp_text_pooler_bwd(const float* grad, const float* y, int relu, const float* h, long long row_stride,
+                           const float* weight, float* dweight, float* dbias, float* dh, int B, int D, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Narrow projection heads: the vid_proj / txt_proj Linear(K, C) of model/model.py:72-79 for widths C the GEMM above
  * cannot take (C % 32 != 0: the OSCC head C = 2, configs/ft/oscc.json; the PNR head C = 16, configs/ft/pnr.json).
  * CUDA-core kernels, no atomics: bitwise reproducible.  All tensors contiguous; K % 8 == 0, 16B-aligned bases.
