@@ -32,13 +32,15 @@ def lib():
         _lib.egovlp_divided_attn_workspace_floats.restype = C.c_longlong
         _lib.egovlp_egonce_fused_workspace_floats.restype = C.c_longlong
         _lib.egovlp_narrow_linear_workspace_floats.restype = C.c_longlong
+        _lib.egovlp_space_attn_long_workspace_floats.restype = C.c_longlong
     return _lib
 
 
 # kernels launched per C-ABI call (memsets excluded) -- bench.py reports the count as `gpu_launches`
 _KERNELS_PER_CALL = {"egovlp_egonce_fused_max_g": 0, "egovlp_divided_attn_fwd": 2, "egovlp_divided_attn_bwd": 2, "egovlp_video_embed_bwd": 2,
                      "egovlp_nce_fwd": 2, "egovlp_dual_softmax": 2, "egovlp_cross_entropy_fwd": 2,
-                     "egovlp_narrow_linear_bwd": 3, "egovlp_text_attn_long_bwd": 3}
+                     "egovlp_narrow_linear_bwd": 3, "egovlp_text_attn_long_bwd": 3, "egovlp_space_attn_long_fwd": 2,
+                     "egovlp_space_attn_long_bwd": 4}
 _launches = 0
 
 

@@ -404,6 +404,25 @@ def _proj_residual(a, pw, pb, resid, cache):
     return out
 
 
+# Most patches per frame the one-CTA-per-frame spatial attention (divided_attn_*, mode 1) takes; larger frames, up to
+# 1024 patches (512 x 512 px at patch 16), run the tiled kernel (space_attn_long_*).  EGOVLP_ATTN_GENERIC and
+# EGOVLP_ATTN_TC select among the divided-attention kernels only, so they do not apply above this.
+SPACE_ATTN_SHORT_MAX_N = 255
+SPACE_ATTN_LONG_MAX_N = 1024
+
+
+def check_video_grid(B, T, N, D, HID):
+    """Refuse, before any launch, a frame the spatial attention cannot take, and a large-frame batch whose widest
+    activation ([B*S, max(3*D, HID)]: qkv or the MLP hidden) has 2^31 elements or more, the range the tower is verified
+    in above N = 255."""
+    if N > SPACE_ATTN_LONG_MAX_N:
+        raise ValueError(f"video tower: {N} patches per frame; the spatial attention takes at most "
+                         f"{SPACE_ATTN_LONG_MAX_N} (512 x 512 px at patch 16)")
+    if N > SPACE_ATTN_SHORT_MAX_N and B * (1 + T * N) * max(3 * D, HID) >= 2 ** 31:
+        raise ValueError(f"video tower: B={B} clips of {T} frames x {N} patches give activations of 2^31 elements or "
+                         f"more ({B * (1 + T * N)} tokens x {max(3 * D, HID)}); split the batch")
+
+
 class SpaceTimeBlockFn(torch.autograd.Function):
     """SpaceTimeBlock.forward (model/video_transformer.py:163-177) incl. both VarAttention calls and the Mlp.
 
@@ -426,6 +445,7 @@ class SpaceTimeBlockFn(torch.autograd.Function):
         S = 1 + T * N
         M = B * S
         HID = f1w.shape[0]
+        check_video_grid(B, T, N, D, HID)
         x2 = x.contiguous().view(M, D)
         # `grad_mode` = torch.is_grad_enabled() at the call site: inside Function.forward grad mode is always off and
         # needs_input_grad reflects requires_grad of the parameters even under torch.no_grad()
@@ -439,7 +459,10 @@ class SpaceTimeBlockFn(torch.autograd.Function):
                 ops.gemm_e4m3(*inp, *cache.get_e4m3(qw), qkv, bias=qb.detach(), col_scale=Q_SCALE, col_scale_ncols=D)
             else:
                 ops.gemm(inp, cache.get(qw), qkv, bias=qb.detach(), col_scale=Q_SCALE, col_scale_ncols=D)
-            a, lse = ops.divided_attn_fwd(qkv, B, T, N, H, mode)
+            if mode == 1 and N > SPACE_ATTN_SHORT_MAX_N:
+                a, lse = ops.space_attn_long_fwd(qkv, B, T, N, H)
+            else:
+                a, lse = ops.divided_attn_fwd(qkv, B, T, N, H, mode)
             return qkv, a, lse, _proj_residual(a, pw, pb, resid, cache)
 
         n3, mean3, rstd3 = ln(x2, n3w, n3b, eps)
@@ -540,7 +563,10 @@ class SpaceTimeBlockFn(torch.autograd.Function):
             g_pw = wgrad(dres16, a, D, D)
             da = _empty((M, D), BF16, dres)
             ops.gemm(dres16, cache.get(pw), da, b_mn=True)
-            dqkv = ops.divided_attn_bwd(qkv, a, da, lse, B, T, N, H, mode, Q_SCALE)
+            if mode == 1 and N > SPACE_ATTN_SHORT_MAX_N:
+                dqkv = ops.space_attn_long_bwd(qkv, a, da, lse, B, T, N, H, Q_SCALE)
+            else:
+                dqkv = ops.divided_attn_bwd(qkv, a, da, lse, B, T, N, H, mode, Q_SCALE)
             g_qw, g_qb = wgrad_and_bgrad(dqkv, inp16, 3 * D, D)
             dinp = _empty((M, D), BF16, dres)
             ops.gemm(dqkv, cache.get(qw), dinp, b_mn=True)

@@ -100,6 +100,21 @@ def _check_bert(tm):
 _VIT_B16_FILE = "pretrained/jx_vit_base_p16_224-80ecf9dd.pth"
 
 
+def resample_pos_embed(pos_embed, grid):
+    """A spatial positional embedding [1, 1 + n*n, D] of a square n x n patch grid, resampled to grid = (rows, cols):
+    the patch part bicubically as a 2-D grid (F.interpolate, align_corners=False, computed in fp32), the CLS entry kept.
+    Returned in pos_embed's dtype, on its device."""
+    n = int(round((pos_embed.shape[1] - 1) ** 0.5))
+    if pos_embed.dim() != 3 or pos_embed.shape[0] != 1 or n * n != pos_embed.shape[1] - 1:
+        raise NotImplementedError(f"pos_embed of shape {tuple(pos_embed.shape)}: only a square patch grid can be "
+                                  "resampled")
+    D = pos_embed.shape[2]
+    patch = pos_embed[:, 1:].float().reshape(1, n, n, D).permute(0, 3, 1, 2)
+    patch = F.interpolate(patch, size=tuple(grid), mode="bicubic", align_corners=False)
+    patch = patch.permute(0, 2, 3, 1).reshape(1, grid[0] * grid[1], D)
+    return torch.cat([pos_embed[:, :1].float(), patch], 1).to(pos_embed.dtype)
+
+
 def _build_video_tower(video_params, from_scratch):
     """SpaceTimeTransformer exactly as the reference configures it (model/model.py:43-66): defaults for missing keys,
     ImageNet ViT-B/16 weights for a tower that is not restored from a checkpoint, identity head / pre_logits / fc."""
@@ -110,7 +125,11 @@ def _build_video_tower(video_params, from_scratch):
     opts.update({k: video_params[k] for k in opts if k in video_params})
     if opts.pop('arch_config') != 'base_patch16_224':
         raise NotImplementedError
-    tower = SpaceTimeTransformer(**opts)
+    # frame size (another key the reference does not read); pretrained pos_embed grids are resampled to it on load
+    img_size = video_params.get('img_size', 224)
+    if isinstance(img_size, bool) or not isinstance(img_size, int) or img_size < 16:
+        raise ValueError(f"video_params['img_size'] must be an int >= 16, got {img_size!r}")
+    tower = SpaceTimeTransformer(img_size=img_size, **opts)
     tower.head = tower.pre_logits = tower.fc = nn.Identity()      # `fc`: "backwards compatibility (old models)"
     # selective activation recompute in training (a key the reference does not read: its configs load unchanged there)
     tower.set_grad_checkpointing(bool(video_params.get('grad_checkpointing', False)))
@@ -118,8 +137,10 @@ def _build_video_tower(video_params, from_scratch):
     tower.set_inference_precision(video_params.get('inference_precision', 'bf16'))
     if from_scratch:
         if os.path.exists(_VIT_B16_FILE):
-            vit = torch.load(_VIT_B16_FILE, map_location="cpu")
-            tower.load_state_dict(state_dict_data_parallel_fix(vit, tower.state_dict()), strict=False)
+            vit = state_dict_data_parallel_fix(torch.load(_VIT_B16_FILE, map_location="cpu"), tower.state_dict())
+            if 'img_size' in video_params and 'pos_embed' in vit:
+                vit['pos_embed'] = resample_pos_embed(vit['pos_embed'], tower.pos_embed_grid())
+            tower.load_state_dict(vit, strict=False)
         else:
             warnings.warn(f"{_VIT_B16_FILE} not found: video tower keeps its random initialisation")
     return tower
@@ -243,7 +264,9 @@ class FrozenInTime(BaseModel):
     # ---- checkpoint compat -----------------------------------------------------------------------------------
     def _inflate_positional_embeds(self, new_state_dict):
         """Load a checkpoint trained with a different number of frames (reference :145-187): truncate, or extend
-        with zeros / nearest / bilinear interpolation along the frame axis."""
+        with zeros / nearest / bilinear interpolation along the frame axis.  A pos_embed of another patch grid is
+        resampled to the tower's (resample_pos_embed) when video_params sets 'img_size'; without that key it is
+        refused, as the reference refuses it."""
         key = 'video_model.temporal_embed'
         curr = self.state_dict()
         if key in new_state_dict and key in curr:
@@ -265,8 +288,10 @@ class FrozenInTime(BaseModel):
                 new_state_dict[key] = new_te
         key = 'video_model.pos_embed'
         if key in new_state_dict and key in curr and new_state_dict[key].shape[1] != curr[key].shape[1]:
-            raise NotImplementedError(
-                'Loading models with different spatial resolution / patch number not yet implemented, sorry.')
+            if 'img_size' not in self.video_params:
+                raise NotImplementedError(
+                    'Loading models with different spatial resolution / patch number not yet implemented, sorry.')
+            new_state_dict[key] = resample_pos_embed(new_state_dict[key], self.video_model.pos_embed_grid())
         return new_state_dict
 
 

@@ -109,7 +109,10 @@ def _default_cache(module):
 
 class SpaceTimeTransformer(nn.Module):
     """Same constructor as the reference (:196-199).  forward(x[B,T,3,H,W]) -> [B, embed_dim] (CLS feature), or
-    head(features) when a classifier head is set."""
+    head(features) when a classifier head is set.  `img_size` (an int or an (H, W) pair) sets the pos_embed grid:
+    any frame of at most 1024 patches runs, e.g. 224 to 512 px or 256 x 320 at patch 16.  Above 255 patches per frame
+    the spatial attention runs on its tiled kernel, which the EGOVLP_ATTN_GENERIC / EGOVLP_ATTN_TC switches do not
+    select; such batches are refused when an activation would reach 2^31 elements (engine.check_video_grid)."""
 
     def __init__(self, img_size=224, patch_size=16, in_chans=3, num_classes=1000, embed_dim=768, depth=12,
                  num_heads=12, mlp_ratio=4., qkv_bias=True, qk_scale=None, representation_size=None,
@@ -156,6 +159,11 @@ class SpaceTimeTransformer(nn.Module):
         self.inference_precision = "bf16"
         object.__setattr__(self, "_bf16_cache", engine.Bf16Cache())
 
+    def pos_embed_grid(self):
+        """(rows, cols) of patches per frame that pos_embed is laid out for."""
+        pe = self.patch_embed
+        return pe.img_size[0] // pe.patch_size[0], pe.img_size[1] // pe.patch_size[1]
+
     def set_grad_checkpointing(self, enable=True):
         """Trade compute for activation memory in training.  This is selective recompute, not timm's re-run of whole
         blocks: each block keeps its input, the qkv and attention outputs, the softmax / LayerNorm statistics and the bf16
@@ -185,11 +193,13 @@ class SpaceTimeTransformer(nn.Module):
         if _refresh and torch.is_grad_enabled():
             cache.refresh()                            # training forward: bf16 weight copies follow ANY optimizer
         pe = self.patch_embed
+        n = (H // pe.patch_size[0]) * (W // pe.patch_size[1])
+        if self.blocks:
+            engine.check_video_grid(B, F, n, self.embed_dim, self.blocks[0].mlp.fc1.out_features)
         # uint8 frames are normalised on the fly with `input_norm` = (mean, std) (default: ImageNet, as the reference's
         # data_loader/transforms.py); float frames are taken as already normalised (the reference contract).
         x = engine.PatchEmbedFn.apply(x, self.cls_token, self.pos_embed, self.temporal_embed, pe.proj.weight,
                                       pe.proj.bias, cache, getattr(self, "input_norm", None))
-        n = (H // pe.patch_size[0]) * (W // pe.patch_size[1])
         for blk in self.blocks:
             x = blk(x, time_n=n, space_f=F, cache=cache, low_memory=self.grad_checkpointing,
                     fp8=self.inference_precision == "fp8")

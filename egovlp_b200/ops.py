@@ -264,6 +264,40 @@ def divided_attn_bwd(qkv, out, dout, lse, B, T, N, H, mode, q_scale, dqkv=None):
     return dqkv
 
 
+def _space_long_ws(B, T, N, H, device):
+    n_ws = lib().egovlp_space_attn_long_workspace_floats(B, T, N, H)
+    assert n_ws > 0, f"space_attn_long: unsupported geometry B={B} T={T} N={N} H={H}"
+    return torch.empty(n_ws, dtype=F32, device=device)
+
+
+def space_attn_long_fwd(qkv, B, T, N, H):
+    """divided_attn_fwd(mode=1) for frames of up to 1024 patches, on the tiled kernel: qkv bf16 [B*S, 3*64*H]
+    (q pre-scaled) -> (out bf16 [B*S, D], lse fp32 [B, H, S])."""
+    _chk(qkv, BF16, "qkv")
+    S, D = 1 + T * N, 64 * H
+    assert qkv.is_contiguous() and qkv.shape == (B * S, 3 * D)
+    out = torch.empty(B * S, D, dtype=BF16, device=qkv.device)
+    lse = torch.empty(B, H, S, dtype=F32, device=qkv.device)
+    ws = _space_long_ws(B, T, N, H, qkv.device)
+    with _Probe("attn_space_long_fwd", B * S * (8 * D + 4 * H)):
+        call("egovlp_space_attn_long_fwd", _ptr(qkv), _ptr(out), _ptr(lse), _ptr(ws), B, T, N, H, _stream())
+    return out, lse
+
+
+def space_attn_long_bwd(qkv, out, dout, lse, B, T, N, H, q_scale, dqkv=None):
+    """Backward of space_attn_long_fwd (out / lse: its outputs) -> dqkv bf16 [B*S, 3*64*H]."""
+    _chk(qkv, BF16, "qkv"); _chk(out, BF16, "out"); _chk(dout, BF16, "dout"); _chk(lse, F32, "lse")
+    assert qkv.is_contiguous() and out.is_contiguous() and dout.is_contiguous() and lse.is_contiguous()
+    if dqkv is None:
+        dqkv = torch.empty_like(qkv)
+    S, D = 1 + T * N, 64 * H
+    ws = _space_long_ws(B, T, N, H, qkv.device)
+    with _Probe("attn_space_long_bwd", B * S * (16 * D + 4 * H)):
+        call("egovlp_space_attn_long_bwd", _ptr(qkv), _ptr(out), _ptr(dout), _ptr(lse), _ptr(dqkv), _ptr(ws), B, T,
+             N, H, C.c_float(q_scale), _stream())
+    return dqkv
+
+
 # ---------------------------------------------------------------- video front end
 def patch_im2col(video, patches, P):
     _chk(video, F32, "video")

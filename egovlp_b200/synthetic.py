@@ -57,9 +57,10 @@ def _bert_shapes(dims, s):
 
 
 def state_dict_shapes(dims, video=True, text=True, proj=True):
-    """Ordered {key: shape} in the reference's registration order."""
+    """Ordered {key: shape} in the reference's registration order.  dims["img"]: an int, or an (H, W) pair."""
     D, H, P = dims["embed_dim"], dims["mlp_hidden"], dims["patch"]
-    n = (dims["img"] // P) ** 2
+    img = dims["img"] if isinstance(dims["img"], (tuple, list)) else (dims["img"], dims["img"])
+    n = (img[0] // P) * (img[1] // P)
     s = OrderedDict()
     if text and dims.get("text_kind") == "bert":
         _bert_shapes(dims, s)
@@ -141,9 +142,11 @@ def seeded_state_dict(dims, seed=0, video=True, text=True, proj=True, dtype=torc
 
 
 def synthetic_video(B, T, seed=0, img=224, device="cpu"):
-    """rand -> ImageNet-normalised, values about U(-2.1, 2.6) (data_loader/transforms.py:38-41)."""
+    """rand -> ImageNet-normalised, values about U(-2.1, 2.6) (data_loader/transforms.py:38-41).  img: an int, or an
+    (H, W) pair."""
     g = torch.Generator().manual_seed(77 + seed)
-    v = torch.rand(B, T, 3, img, img, generator=g)
+    hw = tuple(img) if isinstance(img, (tuple, list)) else (img, img)
+    v = torch.rand(B, T, 3, *hw, generator=g)
     mean = torch.tensor(IMAGENET_MEAN).view(1, 1, 3, 1, 1)
     std = torch.tensor(IMAGENET_STD).view(1, 1, 3, 1, 1)
     return ((v - mean) / std).to(device)

@@ -130,6 +130,20 @@ int egovlp_divided_attn_fwd(const void* qkv, void* out, float* lse, float* cls_p
                             int mode, void* stream);
 int egovlp_divided_attn_bwd(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv,
                             float* dcls_ws, int B, int T, int N, int H, int mode, float q_scale, void* stream);
+/* Spatial attention for large frames: egovlp_divided_attn_{fwd,bwd} with mode = 1 (model/video_transformer.py:109-130,
+ * space mode), for 1 <= N <= 1024 patches per frame (the divided attention stops at N = 255; the engine uses these
+ * above that).  Same qkv / out / lse / dqkv layouts and semantics; tiled on the tensor cores (bf16 mma.sync, fp32
+ * online softmax, 64-row tiles of a frame's rows behind the CLS row).  workspace: fp32, at least
+ * egovlp_space_attn_long_workspace_floats() floats, shared by the forward and the backward (CLS-row partials; the
+ * backward's delta = rowsum(dO * O)).  No floating-point atomics: out, lse and dqkv, the CLS rows included, are
+ * bitwise reproducible, and a sample's results do not depend on the others in the batch.  Indexing is 64-bit.
+ * Refused (EGOVLP_ERR_ARG, nothing written): a null pointer, N outside [1, 1024], B, T or H < 1, B*T or H > 65535.
+ * The workspace query returns -1 for such a shape. */
+long long egovlp_space_attn_long_workspace_floats(int B, int T, int N, int H);
+int egovlp_space_attn_long_fwd(const void* qkv, void* out, float* lse, float* workspace, int B, int T, int N, int H,
+                               void* stream);
+int egovlp_space_attn_long_bwd(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv,
+                               float* workspace, int B, int T, int N, int H, float q_scale, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Video patch-embedding front end (model/video_transformer.py:72-77, 304-321).
