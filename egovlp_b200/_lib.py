@@ -14,7 +14,8 @@ class GemmEpilogue(C.Structure):
                 ("out2", C.c_void_p), ("ldr", C.c_longlong), ("ldaux", C.c_longlong), ("ldo", C.c_longlong),
                 ("ldo2", C.c_longlong), ("out_mode", C.c_int), ("act", C.c_int), ("alpha", C.c_float),
                 ("col_scale", C.c_float), ("col_scale_ncols", C.c_int), ("res_row_mod", C.c_int), ("colsum", C.c_void_p),
-                ("colsum_a", C.c_void_p)]
+                ("colsum_a", C.c_void_p), ("drop_p", C.c_float), ("drop_site", C.c_uint), ("drop_seed", C.c_ulonglong),
+                ("path_p", C.c_float), ("path_site", C.c_uint), ("path_rows", C.c_int)]
 
 
 class EgovlpError(RuntimeError):

@@ -129,6 +129,14 @@ __device__ __forceinline__ uint32_t dropout_threshold(float p) {
   const double t = (double)p * 4294967296.0;
   return t >= 4294967295.0 ? 0xFFFFFFFFu : (uint32_t)t;
 }
+// drop-path (stochastic depth) factor of sample b: 1 / (1 - p) if word (b & 3) of
+// philox4x32_10(dropout_key(seed, site), b / 4) >= dropout_threshold(p), else 0 -- what egovlp_dropout makes of a vector
+// of ones at element b
+__device__ __forceinline__ float drop_path_factor(unsigned long long seed, uint32_t site, float p, long long b) {
+  const uint4 r = philox4x32_10(dropout_key(seed, site), (unsigned long long)(b >> 2));
+  const uint32_t w = (b & 3) == 0 ? r.x : (b & 3) == 1 ? r.y : (b & 3) == 2 ? r.z : r.w;
+  return w >= dropout_threshold(p) ? 1.f / (1.f - p) : 0.f;
+}
 
 // ------------------------------------------------------------------------------------------
 // mma.sync m16n8k16 (bf16 in, fp32 accumulate) on 128B-swizzled [rows x 64] bf16 tiles: row r's 16-byte chunk c sits

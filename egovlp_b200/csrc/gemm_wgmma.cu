@@ -30,6 +30,8 @@
 // unit's fp32 partial tile is added into dW by TMA reduce.  The generic epilogue loads and stores from registers.
 // The same kernel with FP8 = true is the e4m3 inference form (egovlp_gemm_e4m3): e4m3 operands with per-row scales of
 // A and per-column scales of B, applied in the staged epilogue.
+// gemm_drop_wgmma_kernel runs the same body with the video tower's training dropouts in five of the staged epilogues
+// (EPI_*_DROP): the Philox keep mask and the per-sample drop-path factor are applied while the tile is in registers.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -66,6 +68,16 @@ struct EpiParams {
   // e4m3 operands only: acc[m, n] * row_scale[m] * w_scale[n] is the product, before the epilogue above
   const float* row_scale;
   const float* w_scale;
+};
+
+// The dropout forms (EPI_*_DROP) only, a kernel parameter of their own: element (m, n) of the [M, N] output is kept iff
+// word n & 3 of philox4x32_10(dropout_key(seed, site), m * (N / 4) + n / 4) >= dropout_threshold(p), and scaled by
+// 1 / (1 - p) x drop_path_factor(seed, path_site, path_p, m / path_rows) (path_rows = 0: no drop-path)
+struct DropParams {
+  unsigned long long seed;
+  float p, path_p;
+  uint32_t site, path_site;
+  int path_rows;
 };
 
 // Specialised epilogues stage through shared memory: each math warpgroup owns EPI_BUFS subtiles of 64 rows x 128 B
@@ -271,17 +283,28 @@ enum EpiMode {
   EPI_GELU_AUX = 7,  // x GELU'(bf16 aux) -> bf16, GELU(aux) -> bf16 out2                (Mlp.fc2 input gradient)
   // the weight gradients (MN-major A and B, split-K): each unit's fp32 partial tile is added into dW by TMA reduce
   EPI_RED_F32 = 8,   // alpha -> fp32 add into out                                      (every wgrad)
+  // the video tower's training dropouts, applied while the tile is in registers: s = (kept ? 1 / (1 - p) : 0) x the
+  // row's drop-path factor, from the Philox stream of DropParams (the mask does not depend on tiling or batch split)
+  EPI_RES_F32_DROP = 9,    // s (acc + bias) + fp32 residual -> fp32                       (proj / fc2 forward)
+  EPI_ACT3_DROP = 10,      // s GELU(v) -> bf16, GELU'(v) -> bf16 out2                     (Mlp.fc1 forward)
+  EPI_ACT1_Z_DROP = 11,    // s GELU(v) -> bf16, pre-activation -> bf16 out2               (Mlp.fc1 forward, low memory)
+  EPI_MUL_AUX_DROP = 12,   // s v aux -> bf16                                              (Mlp.fc2 input gradient)
+  EPI_GELU_AUX_DROP = 13,  // s v GELU'(aux) -> bf16, s GELU(aux) -> bf16 out2             (the same, low memory)
 };
+// the form a dropout form applies its mask to
+__host__ __device__ constexpr int base_mode(int mode) {
+  return mode == EPI_RES_F32_DROP ? EPI_RES_F32 : mode == EPI_ACT3_DROP ? EPI_ACT3 : mode == EPI_ACT1_Z_DROP ? EPI_ACT1_Z
+       : mode == EPI_MUL_AUX_DROP ? EPI_MUL_AUX : mode == EPI_GELU_AUX_DROP ? EPI_GELU_AUX : mode;
+}
 
 // FP8: A and B are e4m3 (K-major both), one k-block = 128 elements = the same 128 B per row as a bf16 k-block, so the
 // TMA boxes, smem descriptors, stage ring and barriers are byte-identical; each k-block runs 4 k32 steps instead of 4
 // k16 steps, and the staged epilogue first multiplies the accumulators by the row and column scales.
 template <int BLOCK_N, bool A_MN, bool B_MN, bool TWO, int MODE, bool FP8>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                       const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmOut2,
-                       const __grid_constant__ CUtensorMap tmIn, int M, int N, int K, int num_m_blocks,
-                       int num_n_blocks, int kb_per_split, int num_splits, EpiParams ep) {
+__device__ __forceinline__ void
+gemm_bf16_wgmma_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmOut, const CUtensorMap& tmOut2,
+                     const CUtensorMap& tmIn, int M, int N, int K, int num_m_blocks, int num_n_blocks, int kb_per_split,
+                     int num_splits, const EpiParams& ep, const DropParams& dp) {
   static_assert(!(TWO && A_MN && B_MN), "the wgrad form (column sums of A) runs on single CTAs");
   static_assert(!FP8 || (!A_MN && !B_MN && !TWO && (MODE == EPI_BF16 || MODE == EPI_ACT1)),
                 "e4m3: K-major operands, single CTAs, the qkv / fc1 inference epilogues");
@@ -297,10 +320,12 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
   // buffers of the warpgroup; EPI_GELU_AUX has both, and stores its second output from the input's buffer once the
   // first output's store has read it, so that the other buffer stays free for the next aux subtile.
   constexpr bool STAGED = MODE != EPI_GENERIC;
-  constexpr bool RED = MODE == EPI_RED_F32;      // no bias row and no input: warp 1 and the bias barriers stay idle
-  constexpr bool OUT_F32 = MODE == EPI_RES_F32 || RED;
-  constexpr bool HAS_IN = MODE == EPI_RES_F32 || MODE == EPI_MUL_AUX || MODE == EPI_GELU_AUX;
-  constexpr bool TWO_OUT = MODE == EPI_ACT3 || MODE == EPI_ACT1_Z || MODE == EPI_GELU_AUX;
+  constexpr int BM = base_mode(MODE);            // a dropout form runs its base form's epilogue, plus the mask
+  constexpr bool DROP = BM != MODE;
+  constexpr bool RED = BM == EPI_RED_F32;        // no bias row and no input: warp 1 and the bias barriers stay idle
+  constexpr bool OUT_F32 = BM == EPI_RES_F32 || RED;
+  constexpr bool HAS_IN = BM == EPI_RES_F32 || BM == EPI_MUL_AUX || BM == EPI_GELU_AUX;
+  constexpr bool TWO_OUT = BM == EPI_ACT3 || BM == EPI_ACT1_Z || BM == EPI_GELU_AUX;
   constexpr bool BOTH_BUFS = TWO_OUT && !HAS_IN;
   constexpr int SUB_COLS = OUT_F32 ? 32 : 64;
   constexpr int NSUB = BLOCK_N / SUB_COLS;
@@ -543,6 +568,21 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
 #pragma unroll
           for (int h = 0; h < 2; ++h) rs[h] = __ldg(ep.row_scale + min(m_row + wq * 16 + (lane >> 2) + 8 * h, M - 1));
         }
+        // DROP: kept elements of this thread's two rows are scaled by rowf = 1 / (1 - p) x the row's drop-path factor
+        float rowf[2] = {1.f, 1.f};
+        unsigned long long dkey = 0ull;
+        uint32_t dthresh = 0u;
+        if constexpr (DROP) {
+          const float inv = 1.f / (1.f - dp.p);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = m_row + wq * 16 + (lane >> 2) + 8 * h;
+            rowf[h] = dp.path_rows ? inv * drop_path_factor(dp.seed, dp.path_site, dp.path_p, row / dp.path_rows)
+                                   : inv;
+          }
+          dkey = dropout_key(dp.seed, dp.site);
+          dthresh = dropout_threshold(dp.p);
+        }
         if (!RED) mbar_wait_nocall(bias_full, tc & 1);
 #pragma unroll
         for (int s = 0; s < NSUB; ++s, ++it) {
@@ -560,6 +600,20 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
               asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(bq.x), "=f"(bq.y) : "r"(sBias + 4 * (8 * j + c2)));
             float2 ws = make_float2(1.f, 1.f);        // FP8: column scales (N % 128 == 0: every column exists)
             if constexpr (FP8) ws = __ldg(reinterpret_cast<const float2*>(ep.w_scale + n0 + 8 * j + c2));
+            uint32_t keep2[2] = {3u, 3u};             // DROP: keep bits of this thread's two columns, per row half
+            if constexpr (DROP) {
+              // lanes 2i and 2i + 1 hold the same four columns of the same two rows: each draws the four keep bits of one
+              // of the rows (one Philox call per four elements) and the pair swaps them
+              const int hh = lane & 1;
+              const int row = m_row + wq * 16 + (lane >> 2) + 8 * hh;
+              const uint4 r = philox4x32_10(dkey, (unsigned long long)row * (unsigned long long)(N >> 2) +
+                                                      (unsigned long long)((n0 + 8 * j + c2) >> 2));
+              const uint32_t mine = (uint32_t)(r.x >= dthresh) | (uint32_t)(r.y >= dthresh) << 1 |
+                                    (uint32_t)(r.z >= dthresh) << 2 | (uint32_t)(r.w >= dthresh) << 3;
+              const uint32_t other = __shfl_xor_sync(0xffffffffu, mine, 1);
+              keep2[0] = ((hh ? other : mine) >> (c2 & 2)) & 3u;
+              keep2[1] = ((hh ? mine : other) >> (c2 & 2)) & 3u;
+            }
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
               const int r = wq * 16 + (lane >> 2) + 8 * h;  // row of the subtile; 16-byte chunks XOR-swizzled by r & 7
@@ -572,43 +626,59 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
               }
               float v0 = __fmaf_rn(a0, ep.alpha, bq.x);
               float v1 = __fmaf_rn(a1, ep.alpha, bq.y);
-              if (MODE == EPI_BF16 && n0 + 8 * j + c2 < ep.col_scale_ncols) {
+              if (BM == EPI_BF16 && n0 + 8 * j + c2 < ep.col_scale_ncols) {
                 v0 = __fmul_rn(v0, ep.col_scale); v1 = __fmul_rn(v1, ep.col_scale);
               }
+              // DROP: the scale of each of the two elements (0 for a dropped one)
+              const float s0 = (keep2[h] & 1u) ? rowf[h] : 0.f, s1 = (keep2[h] & 2u) ? rowf[h] : 0.f;
               if (BOTH_BUFS) {                  // ACT3: out = GELU(v), out2 = GELU'(v);  ACT1_Z: out = GELU(v), out2 = v
                 uint32_t g, d;
-                if (MODE == EPI_ACT3) {
-                  gelu_and_grad2(gc, v0, v1, g, d);
+                if (BM == EPI_ACT3) {
+                  if constexpr (DROP) {
+                    float g0, g1, d0, d1;
+                    gelu_pair2(gc, v0, v1, g0, g1, d0, d1);
+                    g = pack_bf16x2(__fmul_rn(g0, s0), __fmul_rn(g1, s1));
+                    d = pack_bf16x2(d0, d1);
+                  } else {
+                    gelu_and_grad2(gc, v0, v1, g, d);
+                  }
                 } else {
                   d = pack_bf16x2(v0, v1);
                   gelu2(gc, v0, v1);
+                  if (DROP) { v0 = __fmul_rn(v0, s0); v1 = __fmul_rn(v1, s1); }
                   g = pack_bf16x2(v0, v1);
                 }
                 asm volatile("st.shared.u32 [%0], %1;" ::"r"(buf + off), "r"(g) : "memory");
                 asm volatile("st.shared.u32 [%0], %1;" ::"r"(buf + EPI_SUB_BYTES + off), "r"(d) : "memory");
-              } else if (MODE == EPI_GELU_AUX) {  // out = v GELU'(z), out2 = GELU(z), z = aux
+              } else if (BM == EPI_GELU_AUX) {  // out = v GELU'(z), out2 = GELU(z), z = aux
                 uint32_t a;
                 asm volatile("ld.shared.u32 %0, [%1];" : "=r"(a) : "r"(buf + off) : "memory");
                 const float2 z = unpack_bf16x2(a);
                 float g0, g1, d0, d1;
                 gelu_pair2(gc, z.x, z.y, g0, g1, d0, d1);
-                asm volatile("st.shared.u32 [%0], %1;" ::"r"(buf + off),
-                             "r"(pack_bf16x2(__fmul_rn(v0, d0), __fmul_rn(v1, d1))) : "memory");
+                float o0 = __fmul_rn(v0, d0), o1 = __fmul_rn(v1, d1);
+                if (DROP) {                     // out2 is fc2's (dropped) input: the weight gradient's operand
+                  o0 = __fmul_rn(o0, s0); o1 = __fmul_rn(o1, s1);
+                  g0 = __fmul_rn(g0, s0); g1 = __fmul_rn(g1, s1);
+                }
+                asm volatile("st.shared.u32 [%0], %1;" ::"r"(buf + off), "r"(pack_bf16x2(o0, o1)) : "memory");
                 second[2 * jj + h] = pack_bf16x2(g0, g1);
               } else if (RED) {
                 asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(buf + off), "f"(v0), "f"(v1) : "memory");
-              } else if (MODE == EPI_RES_F32) {
+              } else if (BM == EPI_RES_F32) {
                 float r0, r1;
                 asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(r0), "=f"(r1) : "r"(buf + off) : "memory");
+                if (DROP) { v0 = __fmul_rn(v0, s0); v1 = __fmul_rn(v1, s1); }
                 v0 += r0; v1 += r1;
                 asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(buf + off), "f"(v0), "f"(v1) : "memory");
               } else {
-                if (MODE == EPI_ACT1) gelu2(gc, v0, v1);
-                if (MODE == EPI_MUL_AUX) {
+                if (BM == EPI_ACT1) gelu2(gc, v0, v1);
+                if (BM == EPI_MUL_AUX) {
                   uint32_t a;
                   asm volatile("ld.shared.u32 %0, [%1];" : "=r"(a) : "r"(buf + off) : "memory");
                   const float2 af = unpack_bf16x2(a);
                   v0 *= af.x; v1 *= af.y;
+                  if (DROP) { v0 = __fmul_rn(v0, s0); v1 = __fmul_rn(v1, s1); }
                 }
                 asm volatile("st.shared.u32 [%0], %1;" ::"r"(buf + off), "r"(pack_bf16x2(v0, v1)) : "memory");
               }
@@ -624,7 +694,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
             bulk_wait_read<0>();
             if (HAS_IN && !TWO_OUT) mbar_arrive(epi_empty + 8 * (mw * EPI_BUFS + b));
           }
-          if constexpr (MODE == EPI_GELU_AUX) {
+          if constexpr (BM == EPI_GELU_AUX) {
             named_bar_sync(1 + mw, 128);      // the first output's store has read the buffer
 #pragma unroll
             for (int jj = 0; jj < SUB_COLS / 8; ++jj)
@@ -717,9 +787,41 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
   if (TWO) cluster_sync_all();      // the peer may still multicast into this CTA's smem or arrive on its barriers
 }
 
+template <int BLOCK_N, bool A_MN, bool B_MN, bool TWO, int MODE, bool FP8>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                       const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmOut2,
+                       const __grid_constant__ CUtensorMap tmIn, int M, int N, int K, int num_m_blocks,
+                       int num_n_blocks, int kb_per_split, int num_splits, EpiParams ep) {
+  static_assert(base_mode(MODE) == MODE, "the dropout forms run as gemm_drop_wgmma_kernel");
+  gemm_bf16_wgmma_body<BLOCK_N, A_MN, B_MN, TWO, MODE, FP8>(tmA, tmB, tmOut, tmOut2, tmIn, M, N, K, num_m_blocks,
+                                                             num_n_blocks, kb_per_split, num_splits, ep, DropParams{});
+}
+// the dropout forms: the same kernel with the mask's parameters
+template <int BLOCK_N, bool B_MN, int MODE>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+gemm_drop_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                       const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmOut2,
+                       const __grid_constant__ CUtensorMap tmIn, int M, int N, int K, int num_m_blocks,
+                       int num_n_blocks, int kb_per_split, int num_splits, EpiParams ep, DropParams dp) {
+  static_assert(base_mode(MODE) != MODE, "dropout forms only");
+  gemm_bf16_wgmma_body<BLOCK_N, false, B_MN, false, MODE, false>(tmA, tmB, tmOut, tmOut2, tmIn, M, N, K, num_m_blocks,
+                                                                  num_n_blocks, kb_per_split, num_splits, ep, dp);
+}
+
+template <int BLOCK_N, bool A_MN, bool B_MN, bool TWO, int MODE, bool FP8>
+constexpr auto kernel_of() {
+  if constexpr (base_mode(MODE) != MODE) {
+    static_assert(!A_MN && !TWO && !FP8, "dropout forms: K-major A, single CTAs, bf16");
+    return gemm_drop_wgmma_kernel<BLOCK_N, B_MN, MODE>;
+  } else {
+    return gemm_bf16_wgmma_kernel<BLOCK_N, A_MN, B_MN, TWO, MODE, FP8>;
+  }
+}
+
 template <int BLOCK_N, bool A_MN, bool B_MN, bool TWO, int MODE = EPI_GENERIC, bool FP8 = false>
 int launch(const void* A, long long lda, const void* B, long long ldb, int M, int N, int K, int splits,
-           const EpiParams& ep, cudaStream_t stream) {
+           const EpiParams& ep, cudaStream_t stream, const DropParams& dp = DropParams{}) {
   using C = Cfg<BLOCK_N>;
   CUtensorMap tmA, tmB;
   int rc;
@@ -737,15 +839,16 @@ int launch(const void* A, long long lda, const void* B, long long ldb, int M, in
   }
   // epilogue subtiles of the staged forms: [64 rows, 128 B] boxes over out / out2 / residual / aux
   constexpr bool STAGED = MODE != EPI_GENERIC;
+  constexpr int BM = base_mode(MODE);
   CUtensorMap tmOut = {}, tmOut2 = {}, tmIn = {};
-  if (MODE == EPI_RES_F32 || MODE == EPI_RED_F32) {
+  if (BM == EPI_RES_F32 || BM == EPI_RED_F32) {
     rc = make_tmap_2d_f32(&tmOut, ep.out, M, N, ep.ldo, EPI_ROWS, 32);
-    if (!rc && MODE == EPI_RES_F32) rc = make_tmap_2d_f32(&tmIn, ep.residual, M, N, ep.ldr, EPI_ROWS, 32);
+    if (!rc && BM == EPI_RES_F32) rc = make_tmap_2d_f32(&tmIn, ep.residual, M, N, ep.ldr, EPI_ROWS, 32);
   } else if (STAGED) {
     rc = make_tmap_2d_bf16(&tmOut, ep.out, M, N, ep.ldo, EPI_ROWS, 64);
-    if (!rc && (MODE == EPI_ACT3 || MODE == EPI_ACT1_Z || MODE == EPI_GELU_AUX))
+    if (!rc && (BM == EPI_ACT3 || BM == EPI_ACT1_Z || BM == EPI_GELU_AUX))
       rc = make_tmap_2d_bf16(&tmOut2, ep.out2, M, N, ep.ldo2, EPI_ROWS, 64);
-    if (!rc && (MODE == EPI_MUL_AUX || MODE == EPI_GELU_AUX))
+    if (!rc && (BM == EPI_MUL_AUX || BM == EPI_GELU_AUX))
       rc = make_tmap_2d_bf16(&tmIn, ep.aux, M, N, ep.ldaux, EPI_ROWS, 64);
   }
   if (rc) return rc;
@@ -757,7 +860,7 @@ int launch(const void* A, long long lda, const void* B, long long ldb, int M, in
   const int kb_per_split = (num_kb + splits - 1) / splits;
   splits = (num_kb + kb_per_split - 1) / kb_per_split;  // no empty splits
   const int units = num_m_blocks * num_n_blocks * splits;
-  auto kern = gemm_bf16_wgmma_kernel<BLOCK_N, A_MN, B_MN, TWO, MODE, FP8>;
+  auto kern = kernel_of<BLOCK_N, A_MN, B_MN, TWO, MODE, FP8>();
   static bool attr_set = false;
   if (!attr_set) {
     EGOVLP_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
@@ -791,8 +894,12 @@ int launch(const void* A, long long lda, const void* B, long long ldb, int M, in
   }
   const int workers = min(units, resident);
   cfg.gridDim = dim3(TWO ? 2 * workers : workers);
-  EGOVLP_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, tmOut, tmOut2, tmIn, M, N, K, num_m_blocks, num_n_blocks,
-                                       kb_per_split, splits, ep));
+  if constexpr (BM != MODE)
+    EGOVLP_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, tmOut, tmOut2, tmIn, M, N, K, num_m_blocks, num_n_blocks,
+                                         kb_per_split, splits, ep, dp));
+  else
+    EGOVLP_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, tmOut, tmOut2, tmIn, M, N, K, num_m_blocks, num_n_blocks,
+                                         kb_per_split, splits, ep));
   return EGOVLP_OK;
 }
 
@@ -814,9 +921,13 @@ inline bool tma_ok(const void* p, long long ld_bytes) {
 // Which specialised epilogue (if any) computes exactly what `ep` asks for; EGOVLP_GEMM_GENERIC_EPI=1 keeps every call on
 // the generic one (the kernel tests run both and compare).  The specialised forms move their epilogue bytes by TMA, so a
 // call whose tensors TMA cannot address (see tma_ok; the bias row is a 1-D bulk copy) takes the generic epilogue.
+inline int specialised_mode(const EpiParams& ep);
 inline int epi_mode(const EpiParams& ep) {
   const char* g = getenv("EGOVLP_GEMM_GENERIC_EPI");
   if (g && g[0] == '1') return EPI_GENERIC;
+  return specialised_mode(ep);
+}
+inline int specialised_mode(const EpiParams& ep) {
   if (ep.colsum || ep.res_row_mod) return EPI_GENERIC;
   if (ep.bias && (reinterpret_cast<uintptr_t>(ep.bias) & 15) != 0) return EPI_GENERIC;
   const bool no_scale = ep.col_scale_ncols == 0;
@@ -867,6 +978,28 @@ int dispatch_mode(int a_mn, int b_mn, const void* A, long long lda, const void* 
   return dispatch_major<BLOCK_N, TWO>(a_mn, b_mn, A, lda, B, ldb, M, N, K, splits, ep, stream);
 }
 
+// The dropout forms exist for the video tower's five training calls only (K-major A; B K-major in the forward, MN-major
+// in the fc2 input gradient), on single CTAs.  There is no generic fallback, as the generic epilogue has no mask: any
+// other descriptor with dropout is refused.
+template <int BLOCK_N>
+int dispatch_drop(int a_mn, int b_mn, const void* A, long long lda, const void* B, long long ldb, int M, int N, int K,
+                  const EpiParams& ep, const DropParams& dp, cudaStream_t stream) {
+  const int m = a_mn ? EPI_GENERIC : specialised_mode(ep);
+  if (!b_mn && m == EPI_RES_F32)
+    return launch<BLOCK_N, false, false, false, EPI_RES_F32_DROP>(A, lda, B, ldb, M, N, K, 1, ep, stream, dp);
+  if (!b_mn && m == EPI_ACT3)
+    return launch<BLOCK_N, false, false, false, EPI_ACT3_DROP>(A, lda, B, ldb, M, N, K, 1, ep, stream, dp);
+  if (!b_mn && m == EPI_ACT1_Z)
+    return launch<BLOCK_N, false, false, false, EPI_ACT1_Z_DROP>(A, lda, B, ldb, M, N, K, 1, ep, stream, dp);
+  if (b_mn && m == EPI_MUL_AUX)
+    return launch<BLOCK_N, false, true, false, EPI_MUL_AUX_DROP>(A, lda, B, ldb, M, N, K, 1, ep, stream, dp);
+  if (b_mn && m == EPI_GELU_AUX)
+    return launch<BLOCK_N, false, true, false, EPI_GELU_AUX_DROP>(A, lda, B, ldb, M, N, K, 1, ep, stream, dp);
+  set_last_error("gemm: dropout needs one of the forms bias + fp32 residual -> fp32 (act 0), GELU with out2 (act 1 / 3) "
+                 "with K-major A and B, or act 4 / 5 with K-major A and MN-major B, with TMA-aligned tensors");
+  return EGOVLP_ERR_UNSUPPORTED;
+}
+
 }  // namespace
 
 }  // namespace egovlp
@@ -899,7 +1032,15 @@ extern "C" int egovlp_gemm_bf16(const void* A, int a_mn_major, long long lda, co
   EGOVLP_CHECK_ARG(!e->colsum_a || (a_mn_major && b_mn_major && N % 256 == 0 && M % 8 == 0 &&
                                     (reinterpret_cast<uintptr_t>(e->colsum_a) & 15) == 0),
                    "gemm: colsum_a needs the MN/MN (wgrad) form with N % 256 == 0, M % 8 == 0 and a 16B-aligned vector");
+  EGOVLP_CHECK_ARG(e->drop_p >= 0.f && e->drop_p < 1.f && e->path_p >= 0.f && e->path_p < 1.f && e->path_rows >= 0,
+                   "gemm: dropout rates must lie in [0, 1) (drop_p=%f path_p=%f), path_rows >= 0", e->drop_p, e->path_p);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (e->drop_p > 0.f || e->path_rows > 0) {
+    EGOVLP_CHECK_ARG(split_k <= 1, "gemm: dropout with split_k > 1");
+    const DropParams dp = {e->drop_seed, e->drop_p, e->path_p, e->drop_site, e->path_site, e->path_rows};
+    if (N % 256 == 0) return dispatch_drop<256>(a_mn_major, b_mn_major, A, lda, B, ldb, M, N, K, ep, dp, st);
+    return dispatch_drop<128>(a_mn_major, b_mn_major, A, lda, B, ldb, M, N, K, ep, dp, st);
+  }
   if (N % 256 == 0 && !a_mn_major && use_pairs())
     return dispatch_mode<256, true>(a_mn_major, b_mn_major, A, lda, B, ldb, M, N, K, split_k, ep, st);
   if (N % 256 == 0) return dispatch_mode<256, false>(a_mn_major, b_mn_major, A, lda, B, ldb, M, N, K, split_k, ep, st);

@@ -311,6 +311,11 @@ def bgrad(dy):
     return db
 
 
+def _wgrad_with_bgrad(dy16, x16, n_out, n_in, db):
+    """(dW, db) of a Linear: `db` when its bias gradient was already summed elsewhere, else summed here from dy16."""
+    return (wgrad(dy16, x16, n_out, n_in), db) if db is not None else wgrad_and_bgrad(dy16, x16, n_out, n_in)
+
+
 def _linear_fwd(act16, w16, b, out):
     """out = act16 w16^T + b for the projection heads (model/model.py:72-79): the wgmma GEMM, or for the widths it cannot
     take (C % 32 != 0, e.g. the OSCC / PNR fine-tuning heads of width 2 / 16) the narrow-head kernels."""
@@ -335,11 +340,49 @@ def _linear_bwd(dout, act16, w16):
 # ----------------------------------------------------------------------------------------------------------
 # video tower
 # ----------------------------------------------------------------------------------------------------------
+def draw_dropout_seed():
+    """The Philox seed of one training forward, from torch's CPU generator (torch.manual_seed makes a run reproducible)."""
+    return int(torch.randint(0, 2 ** 62, (1,)).item())
+
+
+# Philox sites of the video tower's training dropouts, all keyed by the one seed its forward draws (masks of the [B*S,
+# width] tensors, element (row, column), as egovlp_dropout draws them; drop-path factors per sample): site 0 = pos_drop
+# on the embedded tokens; block i uses 1 + 6 i + one of the offsets below.
+VIDEO_SITE_POS = 0
+(VIDEO_SITE_TIME_PROJ, VIDEO_SITE_SPACE_PROJ, VIDEO_SITE_GELU, VIDEO_SITE_FC2, VIDEO_SITE_PATH_SPACE,
+ VIDEO_SITE_PATH_MLP) = range(6)
+
+
+def video_block_site(block, offset):
+    return 1 + 6 * block + offset
+
+
+class VideoBlockDrop:
+    """The dropouts of one SpaceTimeBlock in training (model/video_transformer.py:36-52, 135-136, 163-177): proj_drop of
+    timeattn and attn, the Mlp's two dropouts and the drop-path of the space and MLP branches, at the block's sites.
+    `sites(S)` -> the ops.Drop of (time proj output, space proj output, GELU output, fc2 output), None where inactive."""
+
+    def __init__(self, seed, block, p_time, p_space, p_mlp, p_path):
+        self.seed, self.block = int(seed), int(block)
+        self.p_time, self.p_space, self.p_mlp, self.p_path = float(p_time), float(p_space), float(p_mlp), float(p_path)
+
+    def sites(self, S):
+        site = functools.partial(video_block_site, self.block)
+        path = self.p_path > 0
+        return (ops.Drop(self.p_time, self.seed, site(VIDEO_SITE_TIME_PROJ)) if self.p_time > 0 else None,
+                ops.Drop(self.p_space, self.seed, site(VIDEO_SITE_SPACE_PROJ), self.p_path, site(VIDEO_SITE_PATH_SPACE),
+                         S if path else 0) if self.p_space > 0 or path else None,
+                ops.Drop(self.p_mlp, self.seed, site(VIDEO_SITE_GELU)) if self.p_mlp > 0 else None,
+                ops.Drop(self.p_mlp, self.seed, site(VIDEO_SITE_FC2), self.p_path, site(VIDEO_SITE_PATH_MLP),
+                         S if path else 0) if self.p_mlp > 0 or path else None)
+
+
 class PatchEmbedFn(torch.autograd.Function):
-    """VideoPatchEmbed + cls/pos/temporal embedding assembly (model/video_transformer.py:72-77, 304-321)."""
+    """VideoPatchEmbed + cls/pos/temporal embedding assembly (model/video_transformer.py:72-77, 304-321), and the
+    training pos_drop (:244, 320-321) when `drop` (an ops.Drop) is given."""
 
     @staticmethod
-    def forward(ctx, video, cls_token, pos_embed, temporal_embed, w, b, cache, norm=None):
+    def forward(ctx, video, cls_token, pos_embed, temporal_embed, w, b, cache, norm=None, drop=None):
         B, T, C, H, W = video.shape
         D, _, P, _ = w.shape
         _clear_twin(w.device)
@@ -358,7 +401,9 @@ class PatchEmbedFn(torch.autograd.Function):
                             temporal_embed.detach().contiguous(), b.detach(), table, T, N, D)
         x = _empty((B * S, D), F32, w)
         ops.gemm(patches, cache.get(w, (D, K)), x, bias=b.detach(), residual=table, res_row_mod=S)
-        ctx.dims = (B, T, N, D, K, temporal_embed.shape[1])
+        if drop is not None:                    # into a new buffer: the dropout kernel's input and output are restrict
+            x = ops.dropout(x, drop.p, drop.seed, drop.site, y32=torch.empty_like(x))[0]
+        ctx.dims, ctx.drop = (B, T, N, D, K, temporal_embed.shape[1]), drop
         ctx.save_for_backward(patches)
         return x.view(B, S, D)
 
@@ -367,7 +412,13 @@ class PatchEmbedFn(torch.autograd.Function):
         (patches,) = ctx.saved_tensors
         B, T, N, D, K, F = ctx.dims
         dx = dx.contiguous().view(-1, D)
-        dx16 = _bf16_of(dx)
+        drop = ctx.drop
+        if drop is None:
+            dx16 = _bf16_of(dx)
+        else:                   # the gradient of the embedding is the masked one; a published twin is of the unmasked
+            _take_twin(dx)
+            dx16 = _empty(dx.shape, BF16, dx)
+            dx = ops.dropout(dx, drop.p, drop.seed, drop.site, y32=torch.empty_like(dx), y16=dx16)[0]
         if K % 32 == 0:
             dw = wgrad(dx16, patches, D, K)
         else:           # the GEMM's N must be a multiple of 32 (K = 432 at P = 12): form dW^T = patches^T dx instead
@@ -377,7 +428,7 @@ class PatchEmbedFn(torch.autograd.Function):
         tmp = _empty(((1 + T * N) * D,), F32, dx)
         ops.video_embed_bwd(dx, tmp, dcls, dpos, dtemp, dbias, B, T, N, D)
         P = int(round((K // 3) ** 0.5))
-        return None, dcls, dpos, dtemp, dw.reshape(D, 3, P, P), dbias, None, None
+        return None, dcls, dpos, dtemp, dw.reshape(D, 3, P, P), dbias, None, None, None
 
 
 def _ln16(inp, w, b, eps):
@@ -397,10 +448,11 @@ def _ln8(inp, w, b, eps):
     return (y8, scale), None, None
 
 
-def _proj_residual(a, pw, pb, resid, cache):
-    """fp32 resid + proj(a): the attention output projection on the bias + fp32 residual GEMM form."""
+def _proj_residual(a, pw, pb, resid, cache, drop=None):
+    """fp32 resid + proj(a): the attention output projection on the bias + fp32 residual GEMM form (with `drop`, an
+    ops.Drop: resid + the dropped projection)."""
     out = _empty(resid.shape, F32, a)
-    ops.gemm(a, cache.get(pw), out, bias=pb.detach(), residual=resid)
+    ops.gemm(a, cache.get(pw), out, bias=pb.detach(), residual=resid, drop=drop)
     return out
 
 
@@ -435,12 +487,15 @@ class SpaceTimeBlockFn(torch.autograd.Function):
     saves x, qkv, the attention outputs, the softmax and LayerNorm statistics and the bf16 fc1 pre-activation z (21,624
     instead of 38,520 bytes per token at D = 768); the backward rebuilds the residuals tr / sr and the LayerNorm outputs
     from them with the forward's own kernels (bit-identical), and GELU(z) / GELU'(z) inside the fc2 input-gradient GEMM.
+    dims[7] = a VideoBlockDrop or None: the block's training dropouts, fused into the proj / fc1 / fc2 GEMM epilogues
+    (EPI_*_DROP); the backward and the low-memory rebuild regenerate the masks from the seed, so none is saved.  A
+    forward with dropout runs the bf16 GEMMs even when fp8 is asked for.
     """
 
     @staticmethod
     def forward(ctx, x, dims, eps, cache, *p):
         (n1w, n1b, sqw, sqb, spw, spb, tqw, tqb, tpw, tpb, n2w, n2b, f1w, f1b, f2w, f2b, n3w, n3b) = p
-        B, T, N, H, grad_mode, low_memory, fp8 = dims
+        B, T, N, H, grad_mode, low_memory, fp8, drop = dims
         D = H * 64
         S = 1 + T * N
         M = B * S
@@ -450,10 +505,12 @@ class SpaceTimeBlockFn(torch.autograd.Function):
         # `grad_mode` = torch.is_grad_enabled() at the call site: inside Function.forward grad mode is always off and
         # needs_input_grad reflects requires_grad of the parameters even under torch.no_grad()
         train = grad_mode and any(ctx.needs_input_grad)
-        fp8 = fp8 and not train
+        drops = drop.sites(S) if drop is not None else (None, None, None, None)
+        d_time, d_space, d_gelu, d_fc2 = drops
+        fp8 = fp8 and not train and drop is None
         ln = _ln8 if fp8 else _ln16
 
-        def attention(inp, qw, qb, pw, pb, mode, resid):
+        def attention(inp, qw, qb, pw, pb, mode, resid, d):
             qkv = _empty((M, 3 * D), BF16, x2)
             if fp8:
                 ops.gemm_e4m3(*inp, *cache.get_e4m3(qw), qkv, bias=qb.detach(), col_scale=Q_SCALE, col_scale_ncols=D)
@@ -463,26 +520,30 @@ class SpaceTimeBlockFn(torch.autograd.Function):
                 a, lse = ops.space_attn_long_fwd(qkv, B, T, N, H)
             else:
                 a, lse = ops.divided_attn_fwd(qkv, B, T, N, H, mode)
-            return qkv, a, lse, _proj_residual(a, pw, pb, resid, cache)
+            return qkv, a, lse, _proj_residual(a, pw, pb, resid, cache, d)
 
         n3, mean3, rstd3 = ln(x2, n3w, n3b, eps)
-        qkv_t, a_t, lse_t, tr = attention(n3, tqw, tqb, tpw, tpb, 0, x2)          # time_residual = x + time_output
+        qkv_t, a_t, lse_t, tr = attention(n3, tqw, tqb, tpw, tpb, 0, x2, d_time)  # time_residual = x + time_output
         n1, mean1, rstd1 = ln(tr, n1w, n1b, eps)
-        qkv_s, a_s, lse_s, sr = attention(n1, sqw, sqb, spw, spb, 1, x2)          # space_residual = x + space_output
+        qkv_s, a_s, lse_s, sr = attention(n1, sqw, sqb, spw, spb, 1, x2, d_space)  # space_residual = x + space_output
         n2, mean2, rstd2 = ln(sr, n2w, n2b, eps)
         h = _empty((M, HID), BF16, x2)
         # training: u = GELU'(fc1 output) for the backward, or in the low-memory mode z = the fc1 output itself (act 1
         # with out2: h is bit-identical to act 3's)
-        u = _empty((M, HID), BF16, x2) if train else None
-        act = (1 if low_memory else _ACT_FWD) if train else 1
+        # (the GELU-output dropout has the act 3 / act 1 + out2 forms only: a dropping forward keeps u even in inference;
+        # its backward is the act 3 / 4 pair whatever EGOVLP_GELU_DERIV says)
+        u = _empty((M, HID), BF16, x2) if train or d_gelu is not None else None
+        act_fwd, act_bwd = (3, 4) if d_gelu is not None else (_ACT_FWD, _ACT_BWD)
+        act = (1 if low_memory else act_fwd) if train or d_gelu is not None else 1
         if fp8:
             ops.gemm_e4m3(*n2, *cache.get_e4m3(f1w), h, bias=f1b.detach(), act=1)
         else:
-            ops.gemm(n2, cache.get(f1w), h, bias=f1b.detach(), act=act, out2=u)
+            ops.gemm(n2, cache.get(f1w), h, bias=f1b.detach(), act=act, out2=u, drop=d_gelu)
         y = _empty((M, D), F32, x2)
-        ops.gemm(h, cache.get(f2w), y, bias=f2b.detach(), residual=sr)
+        ops.gemm(h, cache.get(f2w), y, bias=f2b.detach(), residual=sr, drop=d_fc2)
         if train:
             ctx.dims, ctx.cache, ctx.eps = (B, T, N, H, HID), cache, eps
+            ctx.drops, ctx.act_bwd = drops, act_bwd
             if low_memory:          # the None slots are rebuilt by the backward (see `rebuild`)
                 ctx.save_for_backward(x2, None, mean3, rstd3, qkv_t, a_t, lse_t, None, None, mean1, rstd1, qkv_s, a_s,
                                       lse_s, None, None, mean2, rstd2, u, None, *p)
@@ -492,17 +553,18 @@ class SpaceTimeBlockFn(torch.autograd.Function):
         return y.view(B, S, D)
 
     @staticmethod
-    def rebuild(which, sv, eps, cache):
+    def rebuild(which, sv, eps, cache, drops=(None, None, None, None)):
         """Rebuild what the low-memory forward did not save, from its saved tensors `sv` (ctx.saved_tensors):
         'sr' -> (space_residual, bf16 norm2(sr)), 'tr' -> (time_residual, bf16 norm1(tr)), 'n3' -> bf16 norm3(x).
-        The proj GEMM and the LayerNorm forward are deterministic, so the results equal the forward's bit for bit."""
+        The proj GEMM and the LayerNorm forward are deterministic, so the results equal the forward's bit for bit; with
+        dropout, `drops` = the forward's ctx.drops regenerates its masks."""
         x2, a_t, a_s, p = sv[0], sv[5], sv[12], sv[20:]
         (n1w, n1b, sqw, sqb, spw, spb, tqw, tqb, tpw, tpb, n2w, n2b, f1w, f1b, f2w, f2b, n3w, n3b) = p
         if which == "sr":
-            r = _proj_residual(a_s, spw, spb, x2, cache)
+            r = _proj_residual(a_s, spw, spb, x2, cache, drops[1])
             return r, _ln16(r, n2w, n2b, eps)[0]
         if which == "tr":
-            r = _proj_residual(a_t, tpw, tpb, x2, cache)
+            r = _proj_residual(a_t, tpw, tpb, x2, cache, drops[0])
             return r, _ln16(r, n1w, n1b, eps)[0]
         if which == "n3":
             return _ln16(x2, n3w, n3b, eps)[0]
@@ -530,21 +592,29 @@ class SpaceTimeBlockFn(torch.autograd.Function):
         (x2, n3, mean3, rstd3, qkv_t, a_t, lse_t, tr, n1, mean1, rstd1, qkv_s, a_s, lse_s, sr, n2, mean2, rstd2, u,
          h) = sv[:20]
         (n1w, n1b, sqw, sqb, spw, spb, tqw, tqb, tpw, tpb, n2w, n2b, f1w, f1b, f2w, f2b, n3w, n3b) = sv[20:]
-        dy16, g_f2b = _byproducts_of(dy)                     # fc2 bias gradient = colsum(dy)
+        d_time, d_space, d_gelu, d_fc2 = ctx.drops
+        # a dropped branch takes dy * mask * drop-path factor / (1 - p) as the bf16 operand of its dgrad, wgrad and bias
+        # gradient; the residual stream keeps dy
+        if d_fc2 is None:
+            dy16, g_f2b = _byproducts_of(dy)                 # fc2 bias gradient = colsum(dy)
+        else:
+            _take_twin(dy)                                   # its twin and column sums are those of the unmasked dy
+            dy16, g_f2b = ops.drop_rows_bf16(dy, d_fc2), None
         low_memory = h is None         # rebuild sr / n2, tr / n1 and n3 as they are consumed; free each after its last use
         if low_memory:
-            sr, n2 = SpaceTimeBlockFn.rebuild("sr", sv, ctx.eps, cache)
+            sr, n2 = SpaceTimeBlockFn.rebuild("sr", sv, ctx.eps, cache, ctx.drops)
 
-        # ---- MLP:  y = sr + fc2(gelu(fc1(LN2(sr))))
+        # ---- MLP:  y = sr + fc2(gelu(fc1(LN2(sr))))   (with dropout: fc2 reads the dropped GELU output h, and its input
+        # gradient is multiplied by the same mask)
         if low_memory:             # u = z: du = (dy W2) * gelu'(z), and the same pass writes h = gelu(z) for the wgrad
             du, h = _empty((M, HID), BF16, dy), _empty((M, HID), BF16, dy)
-            ops.gemm(dy16, cache.get(f2w), du, b_mn=True, aux=u, act=5, out2=h)
-            g_f2w = wgrad(dy16, h, D, HID)
+            ops.gemm(dy16, cache.get(f2w), du, b_mn=True, aux=u, act=5, out2=h, drop=d_gelu)
+            g_f2w, g_f2b = _wgrad_with_bgrad(dy16, h, D, HID, g_f2b)
             del h
         else:
-            g_f2w = wgrad(dy16, h, D, HID)
+            g_f2w, g_f2b = _wgrad_with_bgrad(dy16, h, D, HID, g_f2b)
             du = _empty((M, HID), BF16, dy)
-            ops.gemm(dy16, cache.get(f2w), du, b_mn=True, aux=u, act=_ACT_BWD)            # (dy W2) * gelu'
+            ops.gemm(dy16, cache.get(f2w), du, b_mn=True, aux=u, act=ctx.act_bwd, drop=d_gelu)   # (dy W2) * gelu'
         g_f1w, g_f1b = wgrad_and_bgrad(du, n2, HID, D)       # fc1 bias gradient = colsum(du), summed inside the wgrad GEMM
         del n2
         dn2 = _empty((M, D), BF16, dy)                       # LayerNorm-input gradients travel as bf16
@@ -553,14 +623,15 @@ class SpaceTimeBlockFn(torch.autograd.Function):
         # gradients that stay inside the block (d space_residual, d time_residual) are kept in bf16 only
         dsr16 = _empty((M, D), BF16, dy)
         g_n2w, g_n2b = _zeros((D,), dy), _zeros((D,), dy)
-        g_spb = _zeros((D,), dy)                             # bias grad of attn.proj = colsum(d space_residual)
+        # bias grad of attn.proj = colsum(d space_residual), or with dropout colsum of the masked gradient
+        g_spb = _zeros((D,), dy) if d_space is None else None
         ops.layernorm_bwd(dn2, sr, n2w.detach(), mean2, rstd2, add1=dy, dx16=dsr16, dgamma=g_n2w, dbeta=g_n2b,
                           colsum_dx=g_spb)
         del dn2, sr
 
-        def attention_bwd(dres16, qkv, a, lse, inp16, qw, pw, mode):
+        def attention_bwd(dres16, qkv, a, lse, inp16, qw, pw, mode, g_pb):
             dres = dres16
-            g_pw = wgrad(dres16, a, D, D)
+            g_pw, g_pb = _wgrad_with_bgrad(dres16, a, D, D, g_pb)
             da = _empty((M, D), BF16, dres)
             ops.gemm(dres16, cache.get(pw), da, b_mn=True)
             if mode == 1 and N > SPACE_ATTN_SHORT_MAX_N:
@@ -570,22 +641,26 @@ class SpaceTimeBlockFn(torch.autograd.Function):
             g_qw, g_qb = wgrad_and_bgrad(dqkv, inp16, 3 * D, D)
             dinp = _empty((M, D), BF16, dres)
             ops.gemm(dqkv, cache.get(qw), dinp, b_mn=True)
-            return g_qw, g_qb, g_pw, dinp
+            return g_qw, g_qb, g_pw, g_pb, dinp
 
         # ---- space attention:  sr = x + proj(attn(LN1(tr)))
         if low_memory:
-            tr, n1 = SpaceTimeBlockFn.rebuild("tr", sv, ctx.eps, cache)
-        g_sqw, g_sqb, g_spw, dn1 = attention_bwd(dsr16, qkv_s, a_s, lse_s, n1, sqw, spw, 1)
-        del n1
+            tr, n1 = SpaceTimeBlockFn.rebuild("tr", sv, ctx.eps, cache, ctx.drops)
+        gs16 = dsr16 if d_space is None else ops.drop_rows_bf16(dsr16, d_space)
+        g_sqw, g_sqb, g_spw, g_spb, dn1 = attention_bwd(gs16, qkv_s, a_s, lse_s, n1, sqw, spw, 1, g_spb)
+        del n1, gs16
         dtr16 = _empty((M, D), BF16, dy)
         g_n1w, g_n1b = _zeros((D,), dy), _zeros((D,), dy)
-        g_tpb = _zeros((D,), dy)                             # bias grad of timeattn.proj = colsum(d time_residual)
+        # bias grad of timeattn.proj = colsum(d time_residual), or with dropout colsum of the masked gradient
+        g_tpb = _zeros((D,), dy) if d_time is None else None
         ops.layernorm_bwd(dn1, tr, n1w.detach(), mean1, rstd1, dx16=dtr16, dgamma=g_n1w, dbeta=g_n1b, colsum_dx=g_tpb)
         del dn1, tr
         # ---- time attention:  tr = x + proj(timeattn(LN3(x)))
         if low_memory:
             n3 = SpaceTimeBlockFn.rebuild("n3", sv, ctx.eps, cache)
-        g_tqw, g_tqb, g_tpw, dn3 = attention_bwd(dtr16, qkv_t, a_t, lse_t, n3, tqw, tpw, 0)
+        gt16 = dtr16 if d_time is None else ops.drop_rows_bf16(dtr16, d_time)
+        g_tqw, g_tqb, g_tpw, g_tpb, dn3 = attention_bwd(gt16, qkv_t, a_t, lse_t, n3, tqw, tpw, 0, g_tpb)
+        del gt16
         del n3
         dx, dx16 = _empty((M, D), F32, dy), _empty((M, D), BF16, dy)
         g_n3w, g_n3b = _zeros((D,), dy), _zeros((D,), dy)

@@ -129,7 +129,9 @@ def _build_video_tower(video_params, from_scratch):
     img_size = video_params.get('img_size', 224)
     if isinstance(img_size, bool) or not isinstance(img_size, int) or img_size < 16:
         raise ValueError(f"video_params['img_size'] must be an int >= 16, got {img_size!r}")
-    tower = SpaceTimeTransformer(img_size=img_size, **opts)
+    # training regularisation of the tower (keys the reference's factory does not pass; its configs load unchanged)
+    drops = {k: float(video_params[k]) for k in ('drop_rate', 'attn_drop_rate', 'drop_path_rate') if k in video_params}
+    tower = SpaceTimeTransformer(img_size=img_size, **opts, **drops)
     tower.head = tower.pre_logits = tower.fc = nn.Identity()      # `fc`: "backwards compatibility (old models)"
     # selective activation recompute in training (a key the reference does not read: its configs load unchanged there)
     tower.set_grad_checkpointing(bool(video_params.get('grad_checkpointing', False)))

@@ -64,9 +64,11 @@ class _Probe:
 
 
 def gemm(a, b, out, *, a_mn=False, b_mn=False, bias=None, residual=None, aux=None, out2=None, act=0, alpha=1.0,
-         col_scale=1.0, col_scale_ncols=0, accumulate=False, split_k=1, res_row_mod=0, colsum=None, colsum_a=None):
+         col_scale=1.0, col_scale_ncols=0, accumulate=False, split_k=1, res_row_mod=0, colsum=None, colsum_a=None,
+         drop=None):
     """out = epi(A @ B^T).  a: [M,K] (or [K,M] if a_mn), b: [N,K] (or [K,N] if b_mn); 2-D, last-dim contiguous.
-    out: bf16 or fp32 [M,N]; accumulate=True -> fp32 atomic add into `out` (required for split_k>1)."""
+    out: bf16 or fp32 [M,N]; accumulate=True -> fp32 atomic add into `out` (required for split_k>1).
+    drop: None or a `Drop`: the epilogue's dropout forms (include/egovlp_b200.h, egovlp_gemm_epilogue.drop_*)."""
     _chk(a, BF16, "a"); _chk(b, BF16, "b")
     assert a.dim() == 2 and b.dim() == 2 and a.stride(1) == 1 and b.stride(1) == 1
     (K, M) = a.shape if a_mn else a.shape[::-1]
@@ -105,6 +107,9 @@ def gemm(a, b, out, *, a_mn=False, b_mn=False, bias=None, residual=None, aux=Non
     if colsum_a is not None:                 # wgrad form only: column sums of A accumulated from the smem tiles
         _chk(colsum_a, F32, "colsum_a"); assert a_mn and b_mn and colsum_a.numel() == M
     e.colsum_a = colsum_a.data_ptr() if colsum_a is not None else None
+    if drop is not None:
+        e.drop_p, e.drop_seed, e.drop_site = drop.p, drop.seed, drop.site
+        e.path_p, e.path_site, e.path_rows = drop.path_p, drop.path_site, drop.path_rows
     with _Probe("gemm", 2.0 * M * N * K):
         call("egovlp_gemm_bf16", _ptr(a), int(a_mn), C.c_longlong(a.stride(0)), _ptr(b), int(b_mn),
              C.c_longlong(b.stride(0)), M, N, K, C.byref(e), split_k, _stream())
@@ -422,6 +427,42 @@ def dropout(x, p, seed, site, add=None, y32=None, y16=None):
     call("egovlp_dropout", _ptr(x), _ptr(add), _ptr(y32), _ptr(y16), C.c_longlong(x.numel()), C.c_float(p),
          C.c_ulonglong(seed), C.c_uint(site), _stream())
     return y32, y16
+
+
+class Drop:
+    """One dropout site of a [rows, W] tensor with an optional per-sample drop-path: element (r, c) is kept with the
+    (seed, site) Philox mask of `egovlp_dropout` and scaled by 1 / (1 - p), times the drop-path factor of sample
+    r // path_rows drawn at (seed, path_site) with rate path_p (path_rows = 0: none)."""
+    __slots__ = ("p", "seed", "site", "path_p", "path_site", "path_rows")
+
+    def __init__(self, p, seed, site, path_p=0.0, path_site=0, path_rows=0):
+        self.p, self.seed, self.site = float(p), int(seed), int(site)
+        self.path_p, self.path_site, self.path_rows = float(path_p), int(path_site), int(path_rows)
+
+
+def drop_rows_bf16(x, drop, y=None):
+    """y bf16 [rows, W] = x * keep / (1 - p) * drop-path factor of the row's sample: the gradient of a branch that a GEMM
+    dropout form masked with `drop`.  x fp32 or bf16 [rows, W], contiguous."""
+    assert x.dtype in (F32, BF16) and x.is_cuda and x.is_contiguous() and x.dim() == 2
+    y = torch.empty(x.shape, dtype=BF16, device=x.device) if y is None else y
+    _chk(y, BF16, "y")
+    assert y.shape == x.shape and y.is_contiguous()
+    call("egovlp_drop_rows_bf16", _ptr(x), int(x.dtype == BF16), _ptr(y), C.c_longlong(x.shape[0]), x.shape[1],
+         C.c_float(drop.p), C.c_ulonglong(drop.seed), C.c_uint(drop.site), C.c_float(drop.path_p),
+         C.c_uint(drop.path_site), drop.path_rows, _stream())
+    return y
+
+
+def dropout_mask(rows, width, p, seed, site, device="cuda"):
+    """fp32 [rows, width] multipliers (0 or 1 / (1 - p)) of the (seed, site) element mask of a [rows, width] tensor: the
+    mask of `dropout` and of the GEMM dropout forms."""
+    ones = torch.ones(rows * width, dtype=F32, device=device)
+    return dropout(ones, p, seed, site, y32=torch.empty_like(ones))[0].view(rows, width)
+
+
+def drop_path_factors(n, p, seed, site, device="cuda"):
+    """fp32 [n] per-sample drop-path factors (0 or 1 / (1 - p)) drawn at (seed, site)."""
+    return dropout_mask(1, (n + 3) // 4 * 4, p, seed, site, device)[0, :n]
 
 
 def relu_rows_fwd(x, row_stride, out, rows, D):

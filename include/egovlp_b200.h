@@ -70,6 +70,22 @@ typedef struct egovlp_gemm_epilogue {
   float* colsum_a; /* optional fp32 [M], only with a_mn_major && b_mn_major (the token-contraction weight gradient
                       dW = dy^T x): ACCUMULATES sum_k A[k, m] = the bias gradient of the same Linear, summed from the
                       A tiles while they sit in shared memory for the MMA (no extra pass over dy) */
+  /* Dropout (the video tower's training forms), active when drop_p > 0 or path_rows > 0: the value v that would be
+   * stored (act 0 + residual: the value before the residual is added; act 1 / 3: gelu_erf(v), not out2; act 4: the
+   * product; act 5: both out and out2) is multiplied by keep(m, n) / (1 - drop_p) x f(m / path_rows).  keep(m, n) = 1
+   * iff word (n & 3) of philox4x32_10(key(drop_seed, drop_site), m * (N / 4) + n / 4) >= drop_p * 2^32 -- the mask
+   * egovlp_dropout draws over the [M, N] output, whatever the tiling; f(b) = the drop-path factor of sample b: 1 / (1 -
+   * path_p) if word (b & 3) of philox4x32_10(key(drop_seed, path_site), b / 4) >= path_p * 2^32, else 0 (f = 1 when
+   * path_rows = 0).  Only five forms take it: act 0 + residual + out_mode 1, act 1 / 3 with out2 (K-major A and B),
+   * act 4 / 5 (K-major A, MN-major B); other descriptors return EGOVLP_ERR_UNSUPPORTED.  Rates in [0, 1).
+   * The library reads every field of the struct: zero-initialise it (e.g. `egovlp_gemm_epilogue e = {0};`) so that
+   * the fields a caller does not use, these included, select nothing. */
+  float drop_p;
+  unsigned int drop_site;
+  unsigned long long drop_seed;
+  float path_p;
+  unsigned int path_site;
+  int path_rows;
 } egovlp_gemm_epilogue;
 
 int egovlp_gemm_bf16(const void* A, int a_mn_major, long long lda, const void* B, int b_mn_major, long long ldb,
@@ -383,6 +399,14 @@ int egovlp_cast_f32_to_bf16(const float* src, void* dst_bf16, long long n, void*
 int egovlp_quantize_rows_e4m3(const float* w, long long ldw, uint8_t* q, float* scale, int rows, int K, void* stream);
 /* out[n] += sum_m dy[m, n]  (bias gradients).  dy bf16 or fp32 [M, N] row stride ld. */
 int egovlp_colsum_accum(const void* dy, int dy_is_fp32, long long ld, float* out, int M, int N, void* stream);
+/* Backward of a GEMM dropout form (egovlp_gemm_epilogue.drop_*): y bf16 [rows, W] = bf16(x[r, c] * keep(r, c) /
+ * (1 - p) * f(r / path_rows)), keep and f drawn exactly as that form draws them for a [rows, W] output (f = 1 when
+ * path_rows = 0): the gradient of the video tower's dropped branches (model/video_transformer.py:36-52, 135-136,
+ * 171-175).  x fp32 (x_is_bf16 = 0) or bf16 [rows, W] contiguous, W % 4 == 0, both aligned to four elements; p and
+ * path_p in [0, 1). */
+int egovlp_drop_rows_bf16(const void* x, int x_is_bf16, void* y_bf16, long long rows, int W, float p,
+                          unsigned long long seed, unsigned int site, float path_p, unsigned int path_site,
+                          int path_rows, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Fused multi-tensor AdamW, HuggingFace transformers.AdamW semantics (run/train_egoclip.py:72-73,
