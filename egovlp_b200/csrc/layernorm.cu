@@ -424,15 +424,19 @@ inline bool ln_pipe_enabled() {
   return on == 1;
 }
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+inline bool aligned8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; }
 
+// Views whose base is not 16-byte (src) / 8-byte (dst) aligned, such as the slices of a Bf16Cache.cat buffer, take
+// the scalar path, as in cast_multi_kernel.
 __global__ void cast_f32_to_bf16_kernel(const float* __restrict__ src, bf16* __restrict__ dst, long long n) {
   const long long stride = (long long)gridDim.x * blockDim.x * 4;
+  const bool vec = (reinterpret_cast<uintptr_t>(src) & 15) == 0 && (reinterpret_cast<uintptr_t>(dst) & 7) == 0;
   for (long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) * 4; i < n; i += stride) {
-    if (i + 3 < n) {
+    if (vec && i + 3 < n) {
       const float4 v = *reinterpret_cast<const float4*>(src + i);
       *reinterpret_cast<uint2*>(dst + i) = make_uint2(pack_bf16x2(v.x, v.y), pack_bf16x2(v.z, v.w));
     } else {
-      for (long long j = i; j < n; ++j) dst[j] = __float2bfloat16(src[j]);
+      for (long long j = i; j < min(n, i + 4); ++j) dst[j] = __float2bfloat16(src[j]);   // this thread's 4 only
     }
   }
 }
@@ -540,6 +544,10 @@ extern "C" int egovlp_layernorm_fwd(const float* x, long long ldx, const float* 
                                     float* rstd, int rows, int D, float eps, void* stream) {
   EGOVLP_CHECK_ARG(x && gamma && beta && (y_bf16 || y_f32), "layernorm_fwd: null pointer");
   EGOVLP_CHECK_ARG(rows >= 0 && D > 0 && D % 4 == 0 && D <= 1024 && ldx % 4 == 0, "layernorm_fwd: bad D=%d ldx=%lld", D, ldx);
+  // every kernel moves whole vectors (float4, 4 x bf16): a base off that alignment is refused here instead of faulting
+  EGOVLP_CHECK_ARG(aligned16(x) && aligned16(add) && aligned16(sum_out) && aligned16(gamma) && aligned16(beta) &&
+                   aligned16(y_f32) && aligned8(y_bf16),
+                   "layernorm_fwd: fp32 operands must be 16-byte aligned and bf16 ones 8-byte aligned");
   if (rows == 0) return EGOVLP_OK;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int nv = (D + 127) / 128;
@@ -557,6 +565,8 @@ extern "C" int egovlp_layernorm_fwd_e4m3(const float* x, long long ldx, const fl
   EGOVLP_CHECK_ARG(rows >= 0 && D > 256 && D % 4 == 0 && D <= 1024 && ldx % 4 == 0,
                    "layernorm_fwd_e4m3: bad D=%d ldx=%lld (256 < D <= 1024, D %% 4 == 0)", D, ldx);
   EGOVLP_CHECK_ARG((reinterpret_cast<uintptr_t>(y8) & 3) == 0, "layernorm_fwd_e4m3: y8 must be 4B aligned");
+  EGOVLP_CHECK_ARG(aligned16(x) && aligned16(gamma) && aligned16(beta) && aligned16(y_f32) && aligned8(y_bf16),
+                   "layernorm_fwd_e4m3: fp32 operands must be 16-byte aligned and bf16 ones 8-byte aligned");
   if (rows == 0) return EGOVLP_OK;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int nv = (D + 127) / 128;
@@ -573,6 +583,10 @@ extern "C" int egovlp_layernorm_bwd(const void* dy, int dy_is_bf16, long long ld
                                     void* stream) {
   EGOVLP_CHECK_ARG(dy && x && gamma && mean && rstd && (dx || dx_bf16), "layernorm_bwd: null pointer");
   EGOVLP_CHECK_ARG(rows >= 0 && D > 0 && D % 4 == 0 && D <= 1024 && ldx % 4 == 0 && lddy % 4 == 0 && lddx % 4 == 0, "layernorm_bwd: bad D=%d", D);
+  EGOVLP_CHECK_ARG((dy_is_bf16 ? aligned8(dy) : aligned16(dy)) && (add1_is_bf16 ? aligned8(add1) : aligned16(add1)) &&
+                   (add2_is_bf16 ? aligned8(add2) : aligned16(add2)) && aligned16(x) && aligned16(gamma) &&
+                   aligned16(dx) && aligned8(dx_bf16),
+                   "layernorm_bwd: fp32 operands must be 16-byte aligned and bf16 ones 8-byte aligned");
   if (rows == 0) return EGOVLP_OK;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int nv = (D + 127) / 128;
@@ -585,7 +599,6 @@ extern "C" int egovlp_layernorm_bwd(const void* dy, int dy_is_bf16, long long ld
 extern "C" int egovlp_cast_f32_to_bf16(const float* src, void* dst_bf16, long long n, void* stream) {
   EGOVLP_CHECK_ARG(src && dst_bf16 && n >= 0, "cast: bad args");
   if (n == 0) return EGOVLP_OK;
-  EGOVLP_CHECK_ARG((reinterpret_cast<uintptr_t>(src) & 15) == 0 && (reinterpret_cast<uintptr_t>(dst_bf16) & 7) == 0, "cast: alignment");
   const long long blocks = (n / 4 + 255) / 256;
   long long g = blocks < 1 ? 1 : blocks;
   if (g > (long long)num_sms() * 16) g = (long long)num_sms() * 16;

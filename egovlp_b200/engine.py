@@ -58,7 +58,8 @@ def _zeros(shape, like):
 
 # Generation counter of "some optimizer stepped": bumped by a global torch.optim post-step hook, so that bf16 copies
 # are rebuilt even when the optimizer wrote through `p.data` (transformers.AdamW 4.x, apex), which does not bump
-# `p._version`.  The fused egovlp_b200.optim.AdamW refreshes the copies itself (same kernel pass) and is exempt.
+# `p._version`.  The fused egovlp_b200.optim.AdamW rewrites the copies itself (same kernel pass) and is exempt, so that
+# `get()` right after its step (an evaluation forward) casts nothing; `refresh()` in a training forward re-casts anyway.
 _GEN = 0
 
 
@@ -76,14 +77,14 @@ except ImportError:                                           # pragma: no cover
 
 
 class _CastEntry:
-    __slots__ = ("ref", "t16", "version", "ptr", "gen", "trusted", "scale")
+    __slots__ = ("ref", "t16", "version", "ptr", "gen", "scale")
 
     def __init__(self, p, t16, scale=None):
         self.ref, self.t16, self.scale = weakref.ref(p), t16, scale         # scale: e4m3 entries only
-        self.version, self.ptr, self.gen, self.trusted = -1, 0, -1, False
+        self.version, self.ptr, self.gen = -1, 0, -1
 
-    def stamp(self, p, trusted=False):
-        self.version, self.ptr, self.gen, self.trusted = p._version, p.data_ptr(), _GEN, trusted
+    def stamp(self, p):
+        self.version, self.ptr, self.gen = p._version, p.data_ptr(), _GEN
 
     def current(self, p):
         return (self.ref() is p and self.version == p._version and self.ptr == p.data_ptr() and self.gen == _GEN
@@ -112,8 +113,9 @@ class Bf16Cache:
     * `get(p)` returns the copy, re-casting when the parameter object, its storage, its version or the global
       optimizer generation changed (entries hold a weak reference, so a recycled `id()` cannot alias a dead parameter).
     * `refresh()` -- called at the top of every TRAINING forward -- re-casts every known copy in ONE launch
-      (egovlp_cast_multi_f32_to_bf16) unless the fused AdamW just wrote it, so an update made through `p.data` by any
-      optimizer / EMA is always seen by the next training step.
+      (egovlp_cast_multi_f32_to_bf16), so an update made through `p.data` by any optimizer / EMA is always seen by the
+      next training step.  That includes copies the fused AdamW has just written: a write through `p.data` after its
+      step leaves no trace (`p._version` stays put), so no copy can be trusted to be current at that point.
     * `get_e4m3(p)` returns (e4m3 [N, K], fp32 [N] per-row scales) of a 2-D weight for the fp8 inference GEMMs, under the
       same invalidation rules; `refresh()` marks those entries stale, so they are re-quantised by the next fp8 forward."""
 
@@ -169,7 +171,7 @@ class Bf16Cache:
         return buf
 
     def refresh(self):
-        """Bring every cached copy up to date with one multi-tensor cast (no-op for copies the fused AdamW just wrote)."""
+        """Bring every cached copy up to date with one multi-tensor cast."""
         for key, ent in list(self._e4m3.items()):
             if ent.ref() is None:
                 del self._e4m3[key]
@@ -184,8 +186,7 @@ class Bf16Cache:
                     del _SHADOWS[key]
                 self._table = None
                 continue
-            if not (ent.trusted and ent.current(p)):
-                live.append((p, ent))
+            live.append((p, ent))
         if not live:
             return
         key = tuple((p.data_ptr(), ent.t16.data_ptr(), p.numel()) for p, ent in live)

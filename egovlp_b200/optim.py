@@ -19,7 +19,10 @@ class AdamW(torch.optim.Optimizer):
     One kernel launch per (param group, step count): HF keeps a step counter PER PARAMETER, so parameters that started
     receiving gradients later (unfrozen mid-run, partial optimizer-state load) get their own bias correction -- they are
     launched as a separate sub-group instead of sharing the first parameter's count.  The bf16 GEMM-operand copies
-    that `engine.Bf16Cache` holds for a parameter are rewritten in the same pass (`shadow_bf16`)."""
+    that `engine.Bf16Cache` holds for a parameter are rewritten in the same pass (`shadow_bf16`): a forward that reads
+    them without `Bf16Cache.refresh()` -- an evaluation right after a step -- finds them current and casts nothing.  A
+    training forward re-casts every copy in `refresh()` regardless, since a write through `p.data` after the step would
+    not show in `p._version`."""
 
     _egovlp_fused = True          # engine's optimizer-step hook: this optimizer keeps the bf16 copies current itself
     _RING = 4                     # pinned staging buffers for the descriptor table (pointers move with zero_grad)
@@ -108,5 +111,5 @@ class AdamW(torch.optim.Optimizer):
                 for p, sh in zip(plist, shadows):
                     torch.autograd.graph.increment_version(p)   # the kernel wrote p.data: autograd / caches must see it
                     if sh is not None:
-                        sh.stamp(p, trusted=True)               # ... and its bf16 copy is already current
+                        sh.stamp(p)                             # ... and its bf16 copy is current for Bf16Cache.get()
         return loss
