@@ -216,7 +216,8 @@ egonce_fused_bwd_kernel(const float* __restrict__ text, const float* __restrict_
   __syncthreads();
   const int a = a0 + warp;                               // this warp's "a" row (global index), valid if warp < na_rows
   for (int b0 = 0; b0 < G; b0 += TR) {
-    load_normalised(Bm, ldb, b0, min(TR, G - b0), G, C, g.eps, &bn[0][0], MAXC + 1, nullptr);
+    const int nb_rows = min(TR, G - b0);
+    load_normalised(Bm, ldb, b0, nb_rows, G, C, g.eps, &bn[0][0], MAXC + 1, nullptr);
     __syncthreads();
     // phase 1: x[a, b] and dX for (warp = a row, lane = b row of the tile)
     float dxv = 0.f;
@@ -232,9 +233,10 @@ egonce_fused_bwd_kernel(const float* __restrict__ text, const float* __restrict_
     }
     dxs[warp][lane] = dxv;
     __syncwarp();
-    // phase 2: d an[a, :] += dX[a, b] * bn[b, :]
+    // phase 2: d an[a, :] += dX[a, b] * bn[b, :], over the rows load_normalised wrote: the rest of bn is stale (left
+    // uninitialised at G < 32), and fmaf(0, NaN, acc) would be NaN.  The skipped terms were fmaf(0, finite, acc) == acc.
     if (warp < na_rows) {
-      for (int bl = 0; bl < TR; ++bl) {
+      for (int bl = 0; bl < nb_rows; ++bl) {
         const float d = dxs[warp][bl];
 #pragma unroll
         for (int k = 0; k < MAXC / 32; ++k)
@@ -281,12 +283,33 @@ FusedGeom make_fused_geom(int G, int C, long long ld_t, long long ld_v, long lon
   return g;
 }
 
+// dynamic shared memory of the forward: tag bits [G][W], tn [TR][C], vn [TR][C + 1], xs [TR][GP], mrow [TR][GP / 32]
+size_t fused_fwd_smem(int G, int C, int W) {
+  const int GP = (G + TR - 1) / TR * TR;
+  return (size_t)G * W * 4 + (size_t)TR * C * 4 + (size_t)TR * (C + 1) * 4 + (size_t)TR * GP * 4 + (size_t)TR * (GP / 32) * 4;
+}
+
 }  // namespace
 }  // namespace egovlp
 
 using namespace egovlp;
 
 extern "C" int egovlp_egonce_fused_max_g(void) { return MAXG; }
+
+// 1 if the forward can take this problem on the current device: the tag bits of every row live in shared memory, so a
+// wide tag vocabulary at large G can exceed the opt-in limit (about 1,500 tag columns at G = 512, C = 256 on an H100).
+extern "C" int egovlp_egonce_fused_supported(int G, int C, int n_verb, int n_noun, int mode) {
+  if (G <= 0 || G > MAXG || C <= 0 || C > MAXC || mode < 0 || mode > 3) return 0;
+  if (mode == 0 || mode == 2) n_verb = 0;
+  if (mode == 0 || mode == 3) n_noun = 0;
+  int dev = 0, optin = 0;
+  cudaFuncAttributes fa;
+  if (cudaGetDevice(&dev) != cudaSuccess ||
+      cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess ||
+      cudaFuncGetAttributes(&fa, egonce_fused_fwd_kernel) != cudaSuccess)
+    return 0;
+  return fused_fwd_smem(G, C, (n_verb + 31) / 32 + (n_noun + 31) / 32) + fa.sharedSizeBytes <= (size_t)optin;
+}
 
 extern "C" long long egovlp_egonce_fused_workspace_floats(int G) {
   const long long tiles = (G + TR - 1) / TR;
@@ -305,8 +328,8 @@ extern "C" int egovlp_egonce_fused_fwd(const float* text, long long ld_t, const 
   if (mode == 0 || mode == 2) n_verb = 0;
   if (mode == 0 || mode == 3) n_noun = 0;
   const FusedGeom g = make_fused_geom(G, C, ld_t, ld_v, ld_verb, n_verb, ld_noun, n_noun, inv_temp, mode, eps);
-  const int GP = (G + TR - 1) / TR * TR, W = g.Wv + g.Wn;
-  const size_t smem = (size_t)G * W * 4 + (size_t)TR * C * 4 + (size_t)TR * (C + 1) * 4 + (size_t)TR * GP * 4 + (size_t)TR * (GP / 32) * 4;
+  const int GP = (G + TR - 1) / TR * TR;
+  const size_t smem = fused_fwd_smem(G, C, g.Wv + g.Wn);
   static size_t attr = 0;
   if (smem > attr) {
     EGOVLP_CHECK_CUDA(cudaFuncSetAttribute(egonce_fused_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

@@ -40,19 +40,22 @@ class EgoNCE(nn.Module):
         """Fused entry: gathered embeddings + multi-hot tags -> loss, without materialising the
         verb/noun similarity matrices (positives from bit-packed tag co-occurrence)."""
         G, Cc = text_embeds.shape
-        if ops.egonce_fused_supported(G, Cc) and video_embeds.shape[1] == Cc:      # ONE kernel per direction
+        mode = self._mode()
+        width = lambda t: t.shape[1] if t is not None else 0
+        if (ops.egonce_fused_supported(G, Cc, width(verb_vec), width(noun_vec), mode)
+                and video_embeds.shape[1] == Cc):                                      # ONE kernel per direction
             f = lambda t: t if (t.dtype == torch.float32 and t.stride(1) == 1) else t.float().contiguous()
-            mode = self._mode()
             return engine.FusedEgoNceFn.apply(f(text_embeds), f(video_embeds), f(verb_vec) if mode in (1, 3) else None,
                                               f(noun_vec) if mode in (1, 2) else None, self.temperature, mode)
-        mask = ops.positives_mask_from_tags(verb_vec, noun_vec, self._mode())           # G > 512: kernel-per-stage path
+        mask = ops.positives_mask_from_tags(verb_vec, noun_vec, mode)    # G > 512 or wide tags: kernel-per-stage path
         x = engine.SimMatrixFn.apply(text_embeds, video_embeds, 1e-8)
         return engine.NceLossFn.apply(x, mask, self.temperature)
 
     def gathered(self, text_local, video_local, verb_local, noun_local, gather, rank, world):
         """Data-parallel entry: local rows in, loss out; the packed all-gather happens inside (engine.GatherEgoNceFn)."""
         G, Cc = text_local.shape[0] * world, text_local.shape[1]
-        if ops.egonce_fused_supported(G, Cc) and video_local.shape[1] == Cc:
+        if (ops.egonce_fused_supported(G, Cc, verb_local.shape[1], noun_local.shape[1], self._mode())
+                and video_local.shape[1] == Cc):
             return engine.GatherEgoNceFn.apply(text_local, video_local, verb_local, noun_local, self.temperature,
                                                self._mode(), gather, rank)
         return None

@@ -615,8 +615,9 @@ def pack_rows4(a, b, c, d):
 _fused_ws = {}
 
 
-def egonce_fused_supported(G, C):
-    return G <= lib().egovlp_egonce_fused_max_g() and C <= 256
+def egonce_fused_supported(G, C, n_verb=0, n_noun=0, mode=0):
+    """Whether the fused EgoNCE kernel takes G rows of width C with these tag widths (those `mode` uses)."""
+    return bool(lib().egovlp_egonce_fused_supported(G, C, n_verb, n_noun, mode))
 
 
 def _rows_view(t, name):

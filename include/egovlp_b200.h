@@ -327,6 +327,9 @@ int egovlp_dual_softmax(const float* sim, float* out, int rows, int cols, float 
 int egovlp_pack_rows4(const float* a, int ca, const float* b, int cb, const float* c, int cc, const float* d, int cd,
                       float* out, int rows, void* stream);
 int egovlp_egonce_fused_max_g(void);
+/* 1 if egovlp_egonce_fused_fwd can launch this problem on the current device, else 0: besides the G and C limits, the
+ * tag bits of all G rows (the widths `mode` uses) must fit in shared memory with the similarity tile. */
+int egovlp_egonce_fused_supported(int G, int C, int n_verb, int n_noun, int mode);
 long long egovlp_egonce_fused_workspace_floats(int G);
 int egovlp_egonce_fused_fwd(const float* text, long long ld_t, const float* video, long long ld_v, const float* verb,
                             long long ld_verb, int n_verb, const float* noun, long long ld_noun, int n_noun, int G, int C,
