@@ -15,7 +15,7 @@ class GemmEpilogue(C.Structure):
                 ("ldo2", C.c_longlong), ("out_mode", C.c_int), ("act", C.c_int), ("alpha", C.c_float),
                 ("col_scale", C.c_float), ("col_scale_ncols", C.c_int), ("res_row_mod", C.c_int), ("colsum", C.c_void_p),
                 ("colsum_a", C.c_void_p), ("drop_p", C.c_float), ("drop_site", C.c_uint), ("drop_seed", C.c_ulonglong),
-                ("path_p", C.c_float), ("path_site", C.c_uint), ("path_rows", C.c_int)]
+                ("path_p", C.c_float), ("path_site", C.c_uint), ("path_rows", C.c_int), ("det_ws", C.c_void_p)]
 
 
 class EgovlpError(RuntimeError):
@@ -34,11 +34,17 @@ def lib():
         _lib.egovlp_egonce_fused_workspace_floats.restype = C.c_longlong
         _lib.egovlp_narrow_linear_workspace_floats.restype = C.c_longlong
         _lib.egovlp_space_attn_long_workspace_floats.restype = C.c_longlong
+        for name in ("egovlp_gemm_det_workspace_floats", "egovlp_layernorm_bwd_det_workspace_floats",
+                     "egovlp_colsum_det_workspace_floats", "egovlp_divided_attn_bwd_det_workspace_floats",
+                     "egovlp_maxmargin_det_workspace_floats"):
+            getattr(_lib, name).restype = C.c_longlong
     return _lib
 
 
 # kernels launched per C-ABI call (memsets excluded) -- bench.py reports the count as `gpu_launches`
 _KERNELS_PER_CALL = {"egovlp_egonce_fused_max_g": 0, "egovlp_divided_attn_fwd": 2, "egovlp_divided_attn_bwd": 2, "egovlp_video_embed_bwd": 2,
+                     "egovlp_divided_attn_bwd_det": 2, "egovlp_video_embed_bwd_det": 3, "egovlp_layernorm_bwd_det": 2,
+                     "egovlp_colsum_accum_det": 2, "egovlp_text_embed_bwd_det": 2, "egovlp_maxmargin_fwd_det": 2,
                      "egovlp_nce_fwd": 2, "egovlp_dual_softmax": 2, "egovlp_cross_entropy_fwd": 2,
                      "egovlp_narrow_linear_bwd": 3, "egovlp_text_attn_long_bwd": 3, "egovlp_space_attn_long_fwd": 2,
                      "egovlp_space_attn_long_bwd": 4}
@@ -52,6 +58,12 @@ def reset_launch_count():
 
 def launch_count():
     return _launches
+
+
+def count_launches(n):
+    """Kernels a call launched beyond its entry in _KERNELS_PER_CALL (those that depend on the arguments)."""
+    global _launches
+    _launches += n
 
 
 def call(name, *args):

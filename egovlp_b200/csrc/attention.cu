@@ -368,7 +368,17 @@ __global__ void cls_merge_kernel(const float* __restrict__ part, bf16* __restric
 // ------------------------------------------------------------------------------------------------------------
 // backward
 // ------------------------------------------------------------------------------------------------------------
-template <int NWARPS, int MINB>
+// One element of this CTA's CLS-row gradient (which: 0 dq, 1 dk, 2 dv): added into dcls[b, h, which] by an fp32 atomic
+// (summed over groups in arrival order), or in the deterministic form (DET) stored once into the slot of (b, h, group,
+// part) -- [B, H, G, parts, 3, 64] -- that cls_grad_finalize_kernel then sums in group, then part, order.
+template <bool DET>
+__device__ __forceinline__ void cls_grad_put(float* dcls, const Geom& G, int b, int h, int g, int parts, int part,
+                                             int which, int col, float v) {
+  if (DET) dcls[((((long long)(b * G.H + h)) * G.G + g) * parts + part) * 3 * HD + which * HD + col] = v;
+  else atomicAdd(dcls + ((long long)(b * G.H + h) * 3 + which) * HD + col, v);
+}
+
+template <int NWARPS, int MINB, bool DET>
 __global__ void __launch_bounds__(NWARPS * 32, MINB)
 divided_attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constant__ CUtensorMap tm_do,
                         const bf16* __restrict__ qkv, const bf16* __restrict__ out, const bf16* __restrict__ dout,
@@ -481,11 +491,10 @@ divided_attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid
       const int rc = G.NP - r0;
       if (rc >= 0 && rc < 16 && (rc & 7) == gq) {
         const bool hi_half = rc >= 8;
-        float* dst = dcls + ((long long)(b * G.H + h) * 3 + 0) * HD;
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
-          atomicAdd(dst + j * 8 + 2 * t, hi_half ? dq[j][2] : dq[j][0]);
-          atomicAdd(dst + j * 8 + 2 * t + 1, hi_half ? dq[j][3] : dq[j][1]);
+          cls_grad_put<DET>(dcls, G, b, h, g, 1, 0, 0, j * 8 + 2 * t, hi_half ? dq[j][2] : dq[j][0]);
+          cls_grad_put<DET>(dcls, G, b, h, g, 1, 0, 0, j * 8 + 2 * t + 1, hi_half ? dq[j][3] : dq[j][1]);
         }
       }
     }
@@ -569,14 +578,12 @@ divided_attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid
       const int rc = G.NP - k0r;
       if (rc >= 0 && rc < 16 && (rc & 7) == gq) {
         const bool hi_half = rc >= 8;
-        float* dstk = dcls + ((long long)(b * G.H + h) * 3 + 1) * HD;
-        float* dstv = dcls + ((long long)(b * G.H + h) * 3 + 2) * HD;
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
-          atomicAdd(dstk + j * 8 + 2 * t, hi_half ? dk[j][2] : dk[j][0]);
-          atomicAdd(dstk + j * 8 + 2 * t + 1, hi_half ? dk[j][3] : dk[j][1]);
-          atomicAdd(dstv + j * 8 + 2 * t, hi_half ? dv[j][2] : dv[j][0]);
-          atomicAdd(dstv + j * 8 + 2 * t + 1, hi_half ? dv[j][3] : dv[j][1]);
+          cls_grad_put<DET>(dcls, G, b, h, g, 1, 0, 1, j * 8 + 2 * t, hi_half ? dk[j][2] : dk[j][0]);
+          cls_grad_put<DET>(dcls, G, b, h, g, 1, 0, 1, j * 8 + 2 * t + 1, hi_half ? dk[j][3] : dk[j][1]);
+          cls_grad_put<DET>(dcls, G, b, h, g, 1, 0, 2, j * 8 + 2 * t, hi_half ? dv[j][2] : dv[j][0]);
+          cls_grad_put<DET>(dcls, G, b, h, g, 1, 0, 2, j * 8 + 2 * t + 1, hi_half ? dv[j][3] : dv[j][1]);
         }
       }
     }
@@ -585,13 +592,17 @@ divided_attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid
   }
 }
 
-// dqkv[b, 0, which*D + h*64 + d] = bf16(dcls[b,h,which,d] * (which == 0 ? q_scale : 1))
+// dqkv[b, 0, which*D + h*64 + d] = bf16(dcls[b,h,which,d] * (which == 0 ? q_scale : 1)), dcls[b,h,which,d] being
+// slot 0 + slot 1 + ... of the `slots` slots [B, H, slots, 3, 64] (one slot: the atomics' sums), added left to right
 __global__ void cls_grad_finalize_kernel(const float* __restrict__ dcls, bf16* __restrict__ dqkv, int B, int H, int S,
-                                         int D, float q_scale) {
+                                         int D, float q_scale, int slots) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= B * H * 3 * HD) return;
   const int d = i % HD, which = (i / HD) % 3, h = (i / (3 * HD)) % H, b = i / (3 * HD * H);
-  const float v = dcls[i] * (which == 0 ? q_scale : 1.f);
+  const float* p = dcls + (long long)(i / (3 * HD)) * slots * 3 * HD + which * HD + d;
+  float acc = p[0];
+  for (int k = 1; k < slots; ++k) acc += p[(long long)k * 3 * HD];
+  const float v = acc * (which == 0 ? q_scale : 1.f);
   dqkv[(long long)b * S * 3 * D + which * D + h * HD + d] = __float2bfloat16(v);
 }
 
@@ -1008,7 +1019,7 @@ __device__ __forceinline__ void bwd_k_chunk(const FastCtx& c, const Smem& sm, co
   }
 }
 
-template <bool TIME, int NWARPS, int MINB>
+template <bool TIME, int NWARPS, int MINB, bool DET>
 __global__ void __launch_bounds__(NWARPS * 32, MINB)
 fast_attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constant__ CUtensorMap tm_do,
                      const bf16* __restrict__ qkv, const bf16* __restrict__ out, const bf16* __restrict__ dout,
@@ -1094,11 +1105,10 @@ fast_attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
       const int rc = c.NP - r0;
       if (rc >= 0 && rc < 16 && (rc & 7) == gq) {
         const bool hi_half = rc >= 8;
-        float* dst = dcls + ((long long)(b * G.H + h) * 3 + 0) * HD;
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
-          atomicAdd(dst + j * 8 + 2 * t, hi_half ? dq[j][2] : dq[j][0]);
-          atomicAdd(dst + j * 8 + 2 * t + 1, hi_half ? dq[j][3] : dq[j][1]);
+          cls_grad_put<DET>(dcls, G, b, h, g, TIME ? NWARPS : 1, max(part, 0), 0, j * 8 + 2 * t, hi_half ? dq[j][2] : dq[j][0]);
+          cls_grad_put<DET>(dcls, G, b, h, g, TIME ? NWARPS : 1, max(part, 0), 0, j * 8 + 2 * t + 1, hi_half ? dq[j][3] : dq[j][1]);
         }
       }
     }
@@ -1123,14 +1133,12 @@ fast_attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
       const int rc = c.NP - k0r;
       if (rc >= 0 && rc < 16 && (rc & 7) == gq) {
         const bool hi_half = rc >= 8;
-        float* dstk = dcls + ((long long)(b * G.H + h) * 3 + 1) * HD;
-        float* dstv = dcls + ((long long)(b * G.H + h) * 3 + 2) * HD;
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
-          atomicAdd(dstk + j * 8 + 2 * t, hi_half ? dk[j][2] : dk[j][0]);
-          atomicAdd(dstk + j * 8 + 2 * t + 1, hi_half ? dk[j][3] : dk[j][1]);
-          atomicAdd(dstv + j * 8 + 2 * t, hi_half ? dv[j][2] : dv[j][0]);
-          atomicAdd(dstv + j * 8 + 2 * t + 1, hi_half ? dv[j][3] : dv[j][1]);
+          cls_grad_put<DET>(dcls, G, b, h, g, TIME ? NWARPS : 1, max(part, 0), 1, j * 8 + 2 * t, hi_half ? dk[j][2] : dk[j][0]);
+          cls_grad_put<DET>(dcls, G, b, h, g, TIME ? NWARPS : 1, max(part, 0), 1, j * 8 + 2 * t + 1, hi_half ? dk[j][3] : dk[j][1]);
+          cls_grad_put<DET>(dcls, G, b, h, g, TIME ? NWARPS : 1, max(part, 0), 2, j * 8 + 2 * t, hi_half ? dv[j][2] : dv[j][0]);
+          cls_grad_put<DET>(dcls, G, b, h, g, TIME ? NWARPS : 1, max(part, 0), 2, j * 8 + 2 * t + 1, hi_half ? dv[j][3] : dv[j][1]);
         }
       }
     }
@@ -1232,9 +1240,12 @@ extern "C" int egovlp_divided_attn_fwd(const void* qkv, void* out, float* lse, f
   return EGOVLP_OK;
 }
 
-extern "C" int egovlp_divided_attn_bwd(const void* qkv, const void* out, const void* dout, const float* lse,
-                                       void* dqkv, float* dcls_ws, int B, int T, int N, int H, int mode,
-                                       float q_scale, void* stream) {
+// det: the deterministic form (dcls_ws = egovlp_divided_attn_bwd_det_workspace_floats floats of per-group slots).  It
+// takes the kernel the geometry selects and ignores EGOVLP_ATTN_GENERIC / EGOVLP_ATTN_TIME_BWD_WARPS, so that the slots
+// (and the order they are summed in) follow from the shapes alone.
+static int divided_attn_bwd_impl(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv,
+                                 float* dcls_ws, int B, int T, int N, int H, int mode, float q_scale, bool det,
+                                 void* stream) {
   EGOVLP_CHECK_ARG(qkv && out && dout && lse && dqkv && dcls_ws, "divided_attn_bwd: null pointer");
   EGOVLP_CHECK_ARG(B > 0 && T > 0 && N > 0 && H > 0 && (mode == 0 || mode == 1), "divided_attn_bwd: bad shape");
   Geom G;
@@ -1245,7 +1256,7 @@ extern "C" int egovlp_divided_attn_bwd(const void* qkv, const void* out, const v
   rc = make_group_tmap(&tmd, dout, G, H);
   if (rc) return rc;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  EGOVLP_CHECK_CUDA(cudaMemsetAsync(dcls_ws, 0, (size_t)B * H * 3 * HD * sizeof(float), st));
+  if (!det) EGOVLP_CHECK_CUDA(cudaMemsetAsync(dcls_ws, 0, (size_t)B * H * 3 * HD * sizeof(float), st));
   const bf16* q = reinterpret_cast<const bf16*>(qkv);
   const bf16* o = reinterpret_cast<const bf16*>(out);
   const bf16* d_o = reinterpret_cast<const bf16*>(dout);
@@ -1257,23 +1268,57 @@ extern "C" int egovlp_divided_attn_bwd(const void* qkv, const void* out, const v
     EGOVLP_CHECK_CUDA(cudaFuncSetAttribute(KERN, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));    \
     KERN<<<grid, W * 32, smem, st>>>(tmq, tmd, q, o, d_o, lse, dq, dcls_ws, q_scale, G, ##__VA_ARGS__);       \
   } while (0)
-  const bool generic = force_generic() || (mode == 0 && !time_fast_ok(G));
-  if (generic) {
-    if (G.NPAD > 128) LAUNCH_BWD((divided_attn_bwd_kernel<7, 2>), 7);
-    else LAUNCH_BWD((divided_attn_bwd_kernel<4, 3>), 4);
+  const bool generic = (!det && force_generic()) || (mode == 0 && !time_fast_ok(G));
+  int slots = 1;
+  if (det) {
+    slots = G.G * (generic || mode == 1 ? 1 : 4);
+    if (generic) {
+      if (G.NPAD > 128) LAUNCH_BWD((divided_attn_bwd_kernel<7, 2, true>), 7);
+      else LAUNCH_BWD((divided_attn_bwd_kernel<4, 3, true>), 4);
+    } else if (mode == 1) {
+      if (G.NPAD > 128) LAUNCH_BWD((fast_attn_bwd_kernel<false, 7, 2, true>), 7, 0);
+      else LAUNCH_BWD((fast_attn_bwd_kernel<false, 4, 3, true>), 4, 0);
+    } else {
+      LAUNCH_BWD((fast_attn_bwd_kernel<true, 4, 3, true>), 4, time_shift(G));
+    }
+  } else if (generic) {
+    if (G.NPAD > 128) LAUNCH_BWD((divided_attn_bwd_kernel<7, 2, false>), 7);
+    else LAUNCH_BWD((divided_attn_bwd_kernel<4, 3, false>), 4);
   } else if (mode == 1) {     // space: 2 CTAs / SM (4 x 26 KB tiles each, no staging)
-    if (G.NPAD > 128) LAUNCH_BWD((fast_attn_bwd_kernel<false, 7, 2>), 7, 0);
-    else LAUNCH_BWD((fast_attn_bwd_kernel<false, 4, 3>), 4, 0);
+    if (G.NPAD > 128) LAUNCH_BWD((fast_attn_bwd_kernel<false, 7, 2, false>), 7, 0);
+    else LAUNCH_BWD((fast_attn_bwd_kernel<false, 4, 3, false>), 4, 0);
   } else {
     const char* we = getenv("EGOVLP_ATTN_TIME_BWD_WARPS");
     const bool w8 = we && we[0] == '8';
-    if (w8) LAUNCH_BWD((fast_attn_bwd_kernel<true, 8, 2>), 8, time_shift(G));
-    else LAUNCH_BWD((fast_attn_bwd_kernel<true, 4, 3>), 4, time_shift(G));
+    if (w8) LAUNCH_BWD((fast_attn_bwd_kernel<true, 8, 2, false>), 8, time_shift(G));
+    else LAUNCH_BWD((fast_attn_bwd_kernel<true, 4, 3, false>), 4, time_shift(G));
   }
 #undef LAUNCH_BWD
   EGOVLP_CHECK_LAUNCH();
   const int n = B * H * 3 * HD;
-  cls_grad_finalize_kernel<<<(n + 255) / 256, 256, 0, st>>>(dcls_ws, reinterpret_cast<bf16*>(dqkv), B, H, G.S, G.D, q_scale);
+  cls_grad_finalize_kernel<<<(n + 255) / 256, 256, 0, st>>>(dcls_ws, reinterpret_cast<bf16*>(dqkv), B, H, G.S, G.D, q_scale,
+                                                             slots);
   EGOVLP_CHECK_LAUNCH();
   return EGOVLP_OK;
+}
+
+extern "C" int egovlp_divided_attn_bwd(const void* qkv, const void* out, const void* dout, const float* lse,
+                                       void* dqkv, float* dcls_ws, int B, int T, int N, int H, int mode,
+                                       float q_scale, void* stream) {
+  return divided_attn_bwd_impl(qkv, out, dout, lse, dqkv, dcls_ws, B, T, N, H, mode, q_scale, false, stream);
+}
+
+// [B, H, groups, parts, 3, 64]: one slot per group, four per group in the fast time kernel (its CLS row is split over
+// its four warps)
+extern "C" long long egovlp_divided_attn_bwd_det_workspace_floats(int B, int T, int N, int H, int mode) {
+  Geom G;
+  if (B <= 0 || H <= 0 || (mode != 0 && mode != 1) || make_geom(G, B, T, N, H, mode)) return -1;
+  const int parts = (mode == 0 && time_fast_ok(G)) ? 4 : 1;
+  return (long long)B * H * G.G * parts * 3 * HD;
+}
+
+extern "C" int egovlp_divided_attn_bwd_det(const void* qkv, const void* out, const void* dout, const float* lse,
+                                           void* dqkv, float* dcls_ws, int B, int T, int N, int H, int mode,
+                                           float q_scale, void* stream) {
+  return divided_attn_bwd_impl(qkv, out, dout, lse, dqkv, dcls_ws, B, T, N, H, mode, q_scale, true, stream);
 }

@@ -16,6 +16,39 @@ void set_last_error(const char* fmt, ...) {
   va_end(ap);
 }
 
+// out_k[i] = ((out_k[i] + part_k[0][i]) + part_k[1][i]) + ... for up to three outputs (part_k = part + k * nparts * n):
+// the fixed-order merge of per-CTA partials.  Eight partials are loaded before they are added, in order, so that the
+// loads overlap while the order of the additions stays that of the partials.
+__global__ void ordered_sum_kernel(const float* __restrict__ part, int nparts, long long n, float* __restrict__ out0,
+                                   float* __restrict__ out1, float* __restrict__ out2) {
+  const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const int k = (int)(j / n);
+  const long long i = j - (long long)k * n;
+  float* out = k == 0 ? out0 : k == 1 ? out1 : out2;
+  if (k > 2 || !out) return;
+  const float* p = part + (long long)k * nparts * n + i;
+  float acc = out[i];
+  int q = 0;
+  for (; q + 8 <= nparts; q += 8) {
+    float v[8];
+#pragma unroll
+    for (int u = 0; u < 8; ++u) v[u] = p[(long long)(q + u) * n];
+#pragma unroll
+    for (int u = 0; u < 8; ++u) acc += v[u];
+  }
+  for (; q < nparts; ++q) acc += p[(long long)q * n];
+  out[i] = acc;
+}
+
+int ordered_sum(const float* part, int nparts, long long n, float* out0, float* out1, float* out2, cudaStream_t st) {
+  const int nout = out2 ? 3 : out1 ? 2 : out0 ? 1 : 0;
+  if (nout == 0 || n <= 0) return EGOVLP_OK;
+  const long long total = nout * n;
+  ordered_sum_kernel<<<(unsigned)((total + 127) / 128), 128, 0, st>>>(part, nparts, n, out0, out1, out2);
+  EGOVLP_CHECK_LAUNCH();
+  return EGOVLP_OK;
+}
+
 int num_sms() {
   static int n = 0;
   if (n == 0) {

@@ -40,6 +40,17 @@ void set_last_error(const char* fmt, ...);
 
 int num_sms();
 
+// The deterministic forms size their grids as for this many SMs on every card, so that the partition of a reduction
+// (and with it the bits of its result) is a function of the shapes alone.
+constexpr int DET_SMS = 132;
+// out_k[i] += part_k[0][i] + part_k[1][i] + ... + part_k[nparts - 1][i], added left to right, for each non-null output
+// k < 3 (part_k = part + k * nparts * n: [3][nparts][n]; a null output is skipped, its slab still occupies its place).
+// One launch: the fixed-order merge of per-CTA partials that replaces fp32 atomics in the deterministic forms.
+int ordered_sum(const float* part, int nparts, long long n, float* out0, float* out1, float* out2, cudaStream_t st);
+inline int ordered_sum(const float* part, int nparts, long long n, float* out, cudaStream_t st) {
+  return ordered_sum(part, nparts, n, out, nullptr, nullptr, st);
+}
+
 // ------------------------------------------------------------------------------------------
 // generic device helpers
 // ------------------------------------------------------------------------------------------

@@ -96,7 +96,8 @@ __global__ void sum_over_batch_kernel(const float* __restrict__ dx, float* __res
 // dpos[1+n] += sum_t tmp[1+tN+n];  dtemporal[t] += sum_n tmp[1+tN+n];  dcls += tmp[0]; dpos[0] += tmp[0];
 // dbias += sum_{s>=1} tmp[s].     blockIdx.y selects the job, thread per (index, d).
 __global__ void embed_reduce_kernel(const float* __restrict__ tmp, float* __restrict__ dcls, float* __restrict__ dpos,
-                                    float* __restrict__ dtemporal, float* __restrict__ dbias, int T, int N, int D) {
+                                    float* __restrict__ dtemporal, float* __restrict__ dbias, int T, int N, int D,
+                                    float* __restrict__ dbias_part) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (blockIdx.y == 0) {            // (n, d)
     if (i >= N * D) return;
@@ -110,7 +111,8 @@ __global__ void embed_reduce_kernel(const float* __restrict__ tmp, float* __rest
     float s = 0.f;
     for (int n = 0; n < N; ++n) s += tmp[(long long)(1 + t * N + n) * D + d];
     dtemporal[(long long)t * D + d] += s;
-    atomicAdd(dbias + d, s);
+    if (dbias_part) dbias_part[(long long)t * D + d] = s;      // deterministic form: summed over t in order after
+    else atomicAdd(dbias + d, s);
   } else {                          // d
     if (i >= D) return;
     dcls[i] += tmp[i];
@@ -163,15 +165,26 @@ extern "C" int egovlp_video_pos_table(const float* cls_token, const float* pos_e
   return EGOVLP_OK;
 }
 
-extern "C" int egovlp_video_embed_bwd(const float* dx, float* tmp_SD, float* dcls, float* dpos, float* dtemporal,
-                                      float* dbias, int B, int T, int N, int D, void* stream) {
+static int video_embed_bwd_impl(const float* dx, float* tmp_SD, float* dcls, float* dpos, float* dtemporal,
+                                float* dbias, float* dbias_part, int B, int T, int N, int D, void* stream) {
   EGOVLP_CHECK_ARG(dx && tmp_SD && dcls && dpos && dtemporal && dbias && D % 4 == 0, "video_embed_bwd: bad args");
   const long long SD = (long long)(1 + T * N) * D;
   sum_over_batch_kernel<<<(unsigned)((SD / 4 + 255) / 256), 256, 0, ST(stream)>>>(dx, tmp_SD, B, SD);
   EGOVLP_CHECK_LAUNCH();
   const int mx = max(N, T) * D;
   dim3 grid((mx + 255) / 256, 3);
-  embed_reduce_kernel<<<grid, 256, 0, ST(stream)>>>(tmp_SD, dcls, dpos, dtemporal, dbias, T, N, D);
+  embed_reduce_kernel<<<grid, 256, 0, ST(stream)>>>(tmp_SD, dcls, dpos, dtemporal, dbias, T, N, D, dbias_part);
   EGOVLP_CHECK_LAUNCH();
-  return EGOVLP_OK;
+  return dbias_part ? ordered_sum(dbias_part, T, D, dbias, ST(stream)) : EGOVLP_OK;
+}
+
+extern "C" int egovlp_video_embed_bwd(const float* dx, float* tmp_SD, float* dcls, float* dpos, float* dtemporal,
+                                      float* dbias, int B, int T, int N, int D, void* stream) {
+  return video_embed_bwd_impl(dx, tmp_SD, dcls, dpos, dtemporal, dbias, nullptr, B, T, N, D, stream);
+}
+
+extern "C" int egovlp_video_embed_bwd_det(const float* dx, float* tmp_SD, float* dcls, float* dpos, float* dtemporal,
+                                          float* dbias, float* ws_TD, int B, int T, int N, int D, void* stream) {
+  EGOVLP_CHECK_ARG(ws_TD, "video_embed_bwd_det: null workspace");
+  return video_embed_bwd_impl(dx, tmp_SD, dcls, dpos, dtemporal, dbias, ws_TD, B, T, N, D, stream);
 }

@@ -68,6 +68,11 @@ struct EpiParams {
   // e4m3 operands only: acc[m, n] * row_scale[m] * w_scale[n] is the product, before the epilogue above
   const float* row_scale;
   const float* w_scale;
+  // deterministic form (out_mode 2 and / or colsum_a): each unit stores its fp32 partial tile to det_ws [splits][Mp][N]
+  // (Mp = M rounded up to the 128-row tile) and its colsum_a partial to det_cs [splits][n-blocks][Mp]; gemm_det_merge_*
+  // then add them into out / colsum_a in split (and n-block) order
+  float* det_ws;
+  float* det_cs;
 };
 
 // The dropout forms (EPI_*_DROP) only, a kernel parameter of their own: element (m, n) of the [M, N] output is kept iff
@@ -437,12 +442,15 @@ gemm_bf16_wgmma_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUten
         const int split = unit / num_tiles, tile = unit - split * num_tiles;
         const int m_blk = tile / num_n_blocks, n_blk = tile - m_blk * num_n_blocks;
         const int kb0 = split * kb_per_split, kb1 = min(num_kb, kb0 + kb_per_split);
+        // the deterministic form counts the k-blocks from the split's first, so that a split's partial is the same
+        // as that of a one-split GEMM over the split's rows
+        const int kb_share0 = ep.det_cs ? kb0 : 0;
         float acc[8];
 #pragma unroll
         for (int j = 0; j < 8; ++j) acc[j] = 0.f;
         for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait_nocall(full_bar + 8 * stage, phase);
-          if (kb % num_n_blocks == n_blk) {     // this unit's share of the k-blocks
+          if ((kb - kb_share0) % num_n_blocks == n_blk) {     // this unit's share of the k-blocks
             const uint32_t slab_base = sA + stage * A_STAGE_BYTES + slab * MN_ATOM_BYTES;
 #pragma unroll 4
             for (int i = 0; i < 16; ++i) {
@@ -468,8 +476,14 @@ gemm_bf16_wgmma_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUten
         }
         const int col = m_blk * BLOCK_M + slab * 64 + chunk * 8;
         if (lane < 8 && col < M) {            // M % 8 == 0 is checked by the host
-          red_add_v4(ep.colsum_a + col, acc[0], acc[1], acc[2], acc[3]);
-          red_add_v4(ep.colsum_a + col + 4, acc[4], acc[5], acc[6], acc[7]);
+          if (ep.det_cs) {
+            float* dst = ep.det_cs + ((long long)split * num_n_blocks + n_blk) * (num_m_blocks * BLOCK_M) + col;
+            *reinterpret_cast<float4*>(dst) = make_float4(acc[0], acc[1], acc[2], acc[3]);
+            *reinterpret_cast<float4*>(dst + 4) = make_float4(acc[4], acc[5], acc[6], acc[7]);
+          } else {
+            red_add_v4(ep.colsum_a + col, acc[0], acc[1], acc[2], acc[3]);
+            red_add_v4(ep.colsum_a + col + 4, acc[4], acc[5], acc[6], acc[7]);
+          }
         }
       }
     } else if (STAGED && !RED && warp == 1) {
@@ -687,7 +701,8 @@ gemm_bf16_wgmma_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUten
           fence_proxy_async_smem();
           named_bar_sync(1 + mw, 128);
           if (leader) {
-            if (RED) tma_reduce_add_2d(&tmOut, buf, n0 + s * SUB_COLS, m_row);
+            if (RED && ep.det_ws) tma_store_2d(&tmOut, buf, n0 + s * SUB_COLS, split * num_m_blocks * TILE_M + m_row);
+            else if (RED) tma_reduce_add_2d(&tmOut, buf, n0 + s * SUB_COLS, m_row);
             else tma_store_2d(&tmOut, buf, n0 + s * SUB_COLS, m_row);
             if (BOTH_BUFS) tma_store_2d(&tmOut2, buf + EPI_SUB_BYTES, n0 + s * SUB_COLS, m_row);
             bulk_commit();
@@ -767,6 +782,9 @@ gemm_bf16_wgmma_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUten
             *reinterpret_cast<uint32_t*>(reinterpret_cast<bf16*>(ep.out) + (long long)row * ep.ldo + col) = pack_bf16x2(v0, v1);
           } else if (ep.out_mode == 1) {
             *reinterpret_cast<float2*>(reinterpret_cast<float*>(ep.out) + (long long)row * ep.ldo + col) = make_float2(v0, v1);
+          } else if (ep.det_ws) {
+            *reinterpret_cast<float2*>(ep.det_ws + ((long long)split * num_m_blocks * TILE_M + row) * N + col) =
+                make_float2(v0, v1);
           } else {
             red_add_v2(reinterpret_cast<float*>(ep.out) + (long long)row * ep.ldo + col, v0, v1);
           }
@@ -809,6 +827,50 @@ gemm_drop_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
                                                                   num_n_blocks, kb_per_split, num_splits, ep, dp);
 }
 
+// The deterministic form's ordered pass: out[m, n] = ((out + P_0) + P_1) + ... + P_{s-1}, P_s the partial tile of
+// split s (float4 over n: N % 32 == 0); colsum_a[m] += Q_0 + Q_1 + ..., Q_s = its n-block partials summed in order.
+__global__ void gemm_det_merge_out_kernel(const float* __restrict__ ws, int splits, int M, int Mp, int N,
+                                          float* __restrict__ out, long long ldo) {
+  const long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) * 4;
+  if (i >= (long long)M * N) return;
+  const int m = (int)(i / N), n = (int)(i % N);
+  float4 acc = *reinterpret_cast<const float4*>(out + m * ldo + n);
+  for (int sp = 0; sp < splits; ++sp) {
+    const float4 p = *reinterpret_cast<const float4*>(ws + ((long long)sp * Mp + m) * N + n);
+    acc.x += p.x; acc.y += p.y; acc.z += p.z; acc.w += p.w;
+  }
+  *reinterpret_cast<float4*>(out + m * ldo + n) = acc;
+}
+__global__ void gemm_det_merge_colsum_kernel(const float* __restrict__ cs, int splits, int nnb, int M, int Mp,
+                                             float* __restrict__ colsum_a) {
+  const int m = blockIdx.x * blockDim.x + threadIdx.x;
+  if (m >= M) return;
+  float acc = colsum_a[m];
+  for (int sp = 0; sp < splits; ++sp) {
+    float q = cs[(long long)sp * nnb * Mp + m];
+    for (int nb = 1; nb < nnb; ++nb) q += cs[((long long)sp * nnb + nb) * Mp + m];
+    acc += q;
+  }
+  colsum_a[m] = acc;
+}
+
+// Split count, rows of one split's slab and floats of the deterministic workspace, as launch() computes them
+struct DetLayout {
+  int splits, Mp, nnb;
+  long long floats;
+};
+inline DetLayout det_layout(int M, int N, int K, int splits) {
+  const int num_kb = (K + BLOCK_K - 1) / BLOCK_K;
+  splits = max(1, min(splits, num_kb));
+  const int kb_per_split = (num_kb + splits - 1) / splits;
+  DetLayout d;
+  d.splits = (num_kb + kb_per_split - 1) / kb_per_split;
+  d.Mp = (M + BLOCK_M - 1) / BLOCK_M * BLOCK_M;
+  d.nnb = N % 256 == 0 ? N / 256 : (N + 127) / 128;
+  d.floats = (long long)d.splits * d.Mp * N + (long long)d.splits * d.nnb * d.Mp;
+  return d;
+}
+
 template <int BLOCK_N, bool A_MN, bool B_MN, bool TWO, int MODE, bool FP8>
 constexpr auto kernel_of() {
   if constexpr (base_mode(MODE) != MODE) {
@@ -823,6 +885,8 @@ template <int BLOCK_N, bool A_MN, bool B_MN, bool TWO, int MODE = EPI_GENERIC, b
 int launch(const void* A, long long lda, const void* B, long long ldb, int M, int N, int K, int splits,
            const EpiParams& ep, cudaStream_t stream, const DropParams& dp = DropParams{}) {
   using C = Cfg<BLOCK_N>;
+  const bool det = ep.det_ws != nullptr || ep.det_cs != nullptr;
+  if (det && TWO) { set_last_error("gemm: the deterministic form runs on single CTAs"); return EGOVLP_ERR_UNSUPPORTED; }
   CUtensorMap tmA, tmB;
   int rc;
   if (FP8) {            // e4m3 bytes: the same [rows, 128 B] boxes as the K-major bf16 maps
@@ -841,7 +905,10 @@ int launch(const void* A, long long lda, const void* B, long long ldb, int M, in
   constexpr bool STAGED = MODE != EPI_GENERIC;
   constexpr int BM = base_mode(MODE);
   CUtensorMap tmOut = {}, tmOut2 = {}, tmIn = {};
-  if (BM == EPI_RES_F32 || BM == EPI_RED_F32) {
+  if (BM == EPI_RED_F32 && ep.det_ws) {        // the split slabs of the workspace, [splits * Mp, N]
+    const DetLayout dl = det_layout(M, N, K, splits);
+    rc = make_tmap_2d_f32(&tmOut, ep.det_ws, (uint64_t)dl.splits * dl.Mp, N, N, EPI_ROWS, 32);
+  } else if (BM == EPI_RES_F32 || BM == EPI_RED_F32) {
     rc = make_tmap_2d_f32(&tmOut, ep.out, M, N, ep.ldo, EPI_ROWS, 32);
     if (!rc && BM == EPI_RES_F32) rc = make_tmap_2d_f32(&tmIn, ep.residual, M, N, ep.ldr, EPI_ROWS, 32);
   } else if (STAGED) {
@@ -900,6 +967,20 @@ int launch(const void* A, long long lda, const void* B, long long ldb, int M, in
   else
     EGOVLP_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, tmOut, tmOut2, tmIn, M, N, K, num_m_blocks, num_n_blocks,
                                          kb_per_split, splits, ep));
+  if (det) {
+    const int Mp = num_m_blocks * TILE_M;
+    if (ep.det_ws) {
+      const long long n4 = (long long)M * N / 4;
+      gemm_det_merge_out_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, stream>>>(
+          ep.det_ws, splits, M, Mp, N, reinterpret_cast<float*>(ep.out), ep.ldo);
+      EGOVLP_CHECK_LAUNCH();
+    }
+    if (ep.det_cs) {
+      gemm_det_merge_colsum_kernel<<<(M + 255) / 256, 256, 0, stream>>>(ep.det_cs, splits, num_n_blocks, M, Mp,
+                                                                        ep.colsum_a);
+      EGOVLP_CHECK_LAUNCH();
+    }
+  }
   return EGOVLP_OK;
 }
 
@@ -1029,6 +1110,15 @@ extern "C" int egovlp_gemm_bf16(const void* A, int a_mn_major, long long lda, co
   ep.colsum = e->colsum;
   ep.colsum_a = e->colsum_a;
   ep.row_scale = ep.w_scale = nullptr;
+  ep.det_ws = ep.det_cs = nullptr;
+  if (e->det_ws) {
+    // deterministic form: partials to the workspace, merged in a fixed order (see egovlp_gemm_det_workspace_floats)
+    EGOVLP_CHECK_ARG(!e->colsum, "gemm: the output column sums (colsum) have no deterministic form");
+    EGOVLP_CHECK_ARG((reinterpret_cast<uintptr_t>(e->det_ws) & 15) == 0, "gemm: det_ws must be 16B aligned");
+    const DetLayout dl = det_layout(M, N, K, max(split_k, 1));
+    if (e->out_mode == 2) ep.det_ws = e->det_ws;
+    if (e->colsum_a) ep.det_cs = e->det_ws + (long long)dl.splits * dl.Mp * N;
+  }
   EGOVLP_CHECK_ARG(!e->colsum_a || (a_mn_major && b_mn_major && N % 256 == 0 && M % 8 == 0 &&
                                     (reinterpret_cast<uintptr_t>(e->colsum_a) & 15) == 0),
                    "gemm: colsum_a needs the MN/MN (wgrad) form with N % 256 == 0, M % 8 == 0 and a 16B-aligned vector");
@@ -1041,10 +1131,15 @@ extern "C" int egovlp_gemm_bf16(const void* A, int a_mn_major, long long lda, co
     if (N % 256 == 0) return dispatch_drop<256>(a_mn_major, b_mn_major, A, lda, B, ldb, M, N, K, ep, dp, st);
     return dispatch_drop<128>(a_mn_major, b_mn_major, A, lda, B, ldb, M, N, K, ep, dp, st);
   }
-  if (N % 256 == 0 && !a_mn_major && use_pairs())
+  if (N % 256 == 0 && !a_mn_major && !e->det_ws && use_pairs())
     return dispatch_mode<256, true>(a_mn_major, b_mn_major, A, lda, B, ldb, M, N, K, split_k, ep, st);
   if (N % 256 == 0) return dispatch_mode<256, false>(a_mn_major, b_mn_major, A, lda, B, ldb, M, N, K, split_k, ep, st);
   return dispatch_mode<128, false>(a_mn_major, b_mn_major, A, lda, B, ldb, M, N, K, split_k, ep, st);
+}
+
+extern "C" long long egovlp_gemm_det_workspace_floats(int M, int N, int K, int split_k) {
+  if (M <= 0 || N <= 0 || K <= 0) return -1;
+  return det_layout(M, N, K, max(split_k, 1)).floats;
 }
 
 extern "C" int egovlp_gemm_e4m3(const void* A8, long long lda, const void* B8, long long ldb, const float* row_scale,

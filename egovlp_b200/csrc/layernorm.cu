@@ -112,7 +112,8 @@ layernorm_bwd_kernel(const void* __restrict__ dy_, int dy16, long long lddy, con
                      const float* __restrict__ gamma, const float* __restrict__ mean, const float* __restrict__ rstd,
                      const void* __restrict__ add1, int add1_16, const void* __restrict__ add2, int add2_16,
                      float* __restrict__ dx, long long lddx, bf16* __restrict__ dx16, float* __restrict__ dgamma,
-                     float* __restrict__ dbeta, float* __restrict__ colsum_dx, int rows, int D) {
+                     float* __restrict__ dbeta, float* __restrict__ colsum_dx, int rows, int D,
+                     float* __restrict__ part) {
   __shared__ float4 acc_g[LNB_WARPS][NV * 32];
   __shared__ float4 acc_b[LNB_WARPS][NV * 32];
   __shared__ float4 acc_o[LNB_WARPS][NV * 32];   // column sums of the output (bias gradient of the producing Linear)
@@ -184,6 +185,12 @@ layernorm_bwd_kernel(const void* __restrict__ dy_, int dy16, long long lddy, con
     float sg = 0.f, sb = 0.f, so = 0.f;
 #pragma unroll
     for (int w = 0; w < LNB_WARPS; ++w) { sg += fg[w * NV * 128 + c]; sb += fb[w * NV * 128 + c]; so += fo[w * NV * 128 + c]; }
+    if (part) {          // deterministic form: this CTA's partials, merged in CTA order by ordered_sum
+      part[(0ll * gridDim.x + blockIdx.x) * D + c] = sg;
+      part[(1ll * gridDim.x + blockIdx.x) * D + c] = sb;
+      part[(2ll * gridDim.x + blockIdx.x) * D + c] = so;
+      continue;
+    }
     if (dgamma) atomicAdd(dgamma + c, sg);
     if (dbeta) atomicAdd(dbeta + c, sb);
     if (colsum_dx) atomicAdd(colsum_dx + c, so);
@@ -221,7 +228,7 @@ layernorm_bwd_pipe_kernel(const uint8_t* __restrict__ dy, int dy16, const float*
                           const float* __restrict__ gamma, const float* __restrict__ mean, const float* __restrict__ rstd,
                           const uint8_t* __restrict__ add1, int add1_16, const uint8_t* __restrict__ add2, int add2_16,
                           float* __restrict__ dx, bf16* __restrict__ dx16, float* __restrict__ dgamma,
-                          float* __restrict__ dbeta, float* __restrict__ colsum_dx, int rows) {
+                          float* __restrict__ dbeta, float* __restrict__ colsum_dx, int rows, float* __restrict__ part) {
   constexpr int D = NV * 128;
   extern __shared__ __align__(128) uint8_t ln_smem[];
   __shared__ __align__(8) unsigned long long full_bar[PIPE_STAGES];
@@ -319,6 +326,12 @@ layernorm_bwd_pipe_kernel(const uint8_t* __restrict__ dy, int dy16, const float*
 #pragma unroll
     for (int w = 0; w < PIPE_R; ++w) {
       sg += fr[(0 * PIPE_R + w) * D + c]; sb += fr[(1 * PIPE_R + w) * D + c]; so += fr[(2 * PIPE_R + w) * D + c];
+    }
+    if (part) {
+      part[(0ll * gridDim.x + blockIdx.x) * D + c] = sg;
+      part[(1ll * gridDim.x + blockIdx.x) * D + c] = sb;
+      part[(2ll * gridDim.x + blockIdx.x) * D + c] = so;
+      continue;
     }
     if (dgamma) atomicAdd(dgamma + c, sg);
     if (dbeta) atomicAdd(dbeta + c, sb);
@@ -445,7 +458,8 @@ __global__ void cast_f32_to_bf16_kernel(const float* __restrict__ src, bf16* __r
 // 4 independent row loads in flight per thread; smem reduce over the 8 row-lanes, one atomicAdd per column per block.
 template <bool FP32>
 __global__ void __launch_bounds__(256)
-colsum_kernel(const void* __restrict__ dy, long long ld, float* __restrict__ out, int M, int N, int rows_per_block) {
+colsum_kernel(const void* __restrict__ dy, long long ld, float* __restrict__ out, int M, int N, int rows_per_block,
+              float* __restrict__ part) {
   constexpr int VEC = FP32 ? 4 : 8;
   __shared__ float red[8][32 * VEC + 1];
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
@@ -479,7 +493,8 @@ colsum_kernel(const void* __restrict__ dy, long long ld, float* __restrict__ out
       float t = 0.f;
 #pragma unroll
       for (int w = 0; w < 8; ++w) t += red[w][c];
-      atomicAdd(out + gc, t);
+      if (part) part[(long long)blockIdx.y * N + gc] = t;      // deterministic form: merged in row-block order
+      else atomicAdd(out + gc, t);
     }
   }
 }
@@ -511,8 +526,17 @@ template <int NV>
 int launch_ln_bwd(const void* dy, int dy16, long long lddy, const float* x, long long ldx, const float* gamma,
                   const float* mean, const float* rstd, const void* add1, int add1_16, const void* add2, int add2_16,
                   float* dx, long long lddx, void* dx16, float* dgamma, float* dbeta, float* colsum_dx, int rows, int D,
-                  cudaStream_t st) {
-  if (ln_pipe_enabled() && D == NV * 128 && ldx == D && lddy == D && (!dx || lddx == D) && rows >= 4096 && aligned16(dy) &&
+                  cudaStream_t st, float* part) {
+  // part (deterministic form): per-CTA partials [3][grid][D], merged in CTA order; the kernel choice ignores
+  // EGOVLP_LN_PIPE and the grid is sized for DET_SMS, so both follow from the shapes, the strides and the 16-byte
+  // alignment of dy / x / add1 / add2 (the pipelined kernel's bulk copies need it) alone
+  const bool det = part != nullptr;
+  const int sms = det ? DET_SMS : num_sms();
+  auto merge = [&](int grid) -> int {
+    if (!det) return EGOVLP_OK;
+    return ordered_sum(part, grid, D, dgamma, dbeta, colsum_dx, st);
+  };
+  if ((det || ln_pipe_enabled()) && D == NV * 128 && ldx == D && lddy == D && (!dx || lddx == D) && rows >= 4096 && aligned16(dy) &&
       aligned16(x) && aligned16(add1) && aligned16(add2)) {
     auto kern = layernorm_bwd_pipe_kernel<NV>;
     const int per_elem = (dy16 ? 2 : 4) + 4 + (add1 ? (add1_16 ? 2 : 4) : 0) + (add2 ? (add2_16 ? 2 : 4) : 0);
@@ -520,18 +544,20 @@ int launch_ln_bwd(const void* dy, int dy16, long long lddy, const float* x, long
     static int attr = 0;
     if (attr < smem) { EGOVLP_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); attr = smem; }
     const int tiles = (rows + PIPE_R - 1) / PIPE_R;
-    kern<<<min(tiles, 2 * num_sms()), PIPE_R * 32, smem, st>>>(
+    const int grid = min(tiles, 2 * sms);
+    kern<<<grid, PIPE_R * 32, smem, st>>>(
         reinterpret_cast<const uint8_t*>(dy), dy16, x, gamma, mean, rstd, reinterpret_cast<const uint8_t*>(add1), add1_16,
-        reinterpret_cast<const uint8_t*>(add2), add2_16, dx, reinterpret_cast<bf16*>(dx16), dgamma, dbeta, colsum_dx, rows);
+        reinterpret_cast<const uint8_t*>(add2), add2_16, dx, reinterpret_cast<bf16*>(dx16), dgamma, dbeta, colsum_dx, rows,
+        part);
     EGOVLP_CHECK_LAUNCH();
-    return EGOVLP_OK;
+    return merge(grid);
   }
-  const int grid = min((rows + LNB_WARPS - 1) / LNB_WARPS, num_sms() * 12);
+  const int grid = min((rows + LNB_WARPS - 1) / LNB_WARPS, sms * 12);
   layernorm_bwd_kernel<NV><<<grid, LNB_WARPS * 32, 0, st>>>(dy, dy16, lddy, x, ldx, gamma, mean, rstd, add1, add1_16, add2,
                                                            add2_16, dx, lddx, reinterpret_cast<bf16*>(dx16), dgamma,
-                                                           dbeta, colsum_dx, rows, D);
+                                                           dbeta, colsum_dx, rows, D, part);
   EGOVLP_CHECK_LAUNCH();
-  return EGOVLP_OK;
+  return merge(grid);
 }
 
 }  // namespace
@@ -576,11 +602,11 @@ extern "C" int egovlp_layernorm_fwd_e4m3(const float* x, long long ldx, const fl
   return EGOVLP_ERR_UNSUPPORTED;
 }
 
-extern "C" int egovlp_layernorm_bwd(const void* dy, int dy_is_bf16, long long lddy, const float* x, long long ldx,
-                                    const float* gamma, const float* mean, const float* rstd, const void* add1,
-                                    int add1_is_bf16, const void* add2, int add2_is_bf16, float* dx, long long lddx,
-                                    void* dx_bf16, float* dgamma, float* dbeta, float* colsum_dx, int rows, int D,
-                                    void* stream) {
+static int layernorm_bwd_impl(const void* dy, int dy_is_bf16, long long lddy, const float* x, long long ldx,
+                              const float* gamma, const float* mean, const float* rstd, const void* add1,
+                              int add1_is_bf16, const void* add2, int add2_is_bf16, float* dx, long long lddx,
+                              void* dx_bf16, float* dgamma, float* dbeta, float* colsum_dx, int rows, int D, float* part,
+                              void* stream) {
   EGOVLP_CHECK_ARG(dy && x && gamma && mean && rstd && (dx || dx_bf16), "layernorm_bwd: null pointer");
   EGOVLP_CHECK_ARG(rows >= 0 && D > 0 && D % 4 == 0 && D <= 1024 && ldx % 4 == 0 && lddy % 4 == 0 && lddx % 4 == 0, "layernorm_bwd: bad D=%d", D);
   EGOVLP_CHECK_ARG((dy_is_bf16 ? aligned8(dy) : aligned16(dy)) && (add1_is_bf16 ? aligned8(add1) : aligned16(add1)) &&
@@ -590,10 +616,39 @@ extern "C" int egovlp_layernorm_bwd(const void* dy, int dy_is_bf16, long long ld
   if (rows == 0) return EGOVLP_OK;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int nv = (D + 127) / 128;
-#define LN_BWD_CASE(n) case n: return launch_ln_bwd<n>(dy, dy_is_bf16, lddy, x, ldx, gamma, mean, rstd, add1, add1_is_bf16, add2, add2_is_bf16, dx, lddx, dx_bf16, dgamma, dbeta, colsum_dx, rows, D, st)
+#define LN_BWD_CASE(n) case n: return launch_ln_bwd<n>(dy, dy_is_bf16, lddy, x, ldx, gamma, mean, rstd, add1, add1_is_bf16, add2, add2_is_bf16, dx, lddx, dx_bf16, dgamma, dbeta, colsum_dx, rows, D, st, part)
   switch (nv) { LN_BWD_CASE(1); LN_BWD_CASE(2); LN_BWD_CASE(3); LN_BWD_CASE(4); LN_BWD_CASE(5); LN_BWD_CASE(6); LN_BWD_CASE(7); LN_BWD_CASE(8); }
 #undef LN_BWD_CASE
   return EGOVLP_ERR_UNSUPPORTED;
+}
+
+extern "C" int egovlp_layernorm_bwd(const void* dy, int dy_is_bf16, long long lddy, const float* x, long long ldx,
+                                    const float* gamma, const float* mean, const float* rstd, const void* add1,
+                                    int add1_is_bf16, const void* add2, int add2_is_bf16, float* dx, long long lddx,
+                                    void* dx_bf16, float* dgamma, float* dbeta, float* colsum_dx, int rows, int D,
+                                    void* stream) {
+  return layernorm_bwd_impl(dy, dy_is_bf16, lddy, x, ldx, gamma, mean, rstd, add1, add1_is_bf16, add2, add2_is_bf16, dx,
+                            lddx, dx_bf16, dgamma, dbeta, colsum_dx, rows, D, nullptr, stream);
+}
+
+// the largest grid either backward kernel takes for these shapes in the deterministic form, x 3 sums x D
+extern "C" long long egovlp_layernorm_bwd_det_workspace_floats(int rows, int D) {
+  if (rows < 0 || D <= 0) return -1;
+  const long long pipe = min((rows + PIPE_R - 1) / PIPE_R, 2 * DET_SMS);
+  const long long gen = min((rows + LNB_WARPS - 1) / LNB_WARPS, 12 * DET_SMS);
+  return 3ll * max(pipe, gen) * D;
+}
+
+extern "C" int egovlp_layernorm_bwd_det(const void* dy, int dy_is_bf16, long long lddy, const float* x, long long ldx,
+                                        const float* gamma, const float* mean, const float* rstd, const void* add1,
+                                        int add1_is_bf16, const void* add2, int add2_is_bf16, float* dx, long long lddx,
+                                        void* dx_bf16, float* dgamma, float* dbeta, float* colsum_dx, int rows, int D,
+                                        float* ws, void* stream) {
+  EGOVLP_CHECK_ARG(ws || (!dgamma && !dbeta && !colsum_dx), "layernorm_bwd_det: null workspace");
+  // without any column sum there is nothing to reduce: the plain kernel is deterministic as it stands
+  const bool sums = dgamma || dbeta || colsum_dx;
+  return layernorm_bwd_impl(dy, dy_is_bf16, lddy, x, ldx, gamma, mean, rstd, add1, add1_is_bf16, add2, add2_is_bf16, dx,
+                            lddx, dx_bf16, dgamma, dbeta, colsum_dx, rows, D, sums ? ws : nullptr, stream);
 }
 
 extern "C" int egovlp_cast_f32_to_bf16(const float* src, void* dst_bf16, long long n, void* stream) {
@@ -642,21 +697,45 @@ extern "C" int egovlp_quantize_rows_e4m3(const float* w, long long ldw, uint8_t*
   return EGOVLP_OK;
 }
 
-extern "C" int egovlp_colsum_accum(const void* dy, int dy_is_fp32, long long ld, float* out, int M, int N,
-                                   void* stream) {
+// The row-block split (sized for DET_SMS when `part` is given: deterministic form, part = [row_blocks][N])
+static void colsum_grid(int M, int N, int vec, int sms, int& row_blocks, int& rows_per_block) {
+  const int col_blocks = (N / vec + 31) / 32;
+  row_blocks = max(1, min((M + 63) / 64, (sms * 8 + col_blocks - 1) / col_blocks));
+  rows_per_block = (M + row_blocks - 1) / row_blocks;
+  row_blocks = (M + rows_per_block - 1) / rows_per_block;
+}
+
+static int colsum_impl(const void* dy, int dy_is_fp32, long long ld, float* out, int M, int N, float* part, void* stream) {
   EGOVLP_CHECK_ARG(dy && out && M >= 0 && N > 0, "colsum: bad args");
   if (M == 0) return EGOVLP_OK;
   const int vec = dy_is_fp32 ? 4 : 8;
   EGOVLP_CHECK_ARG(N % vec == 0 && ld % vec == 0 && (reinterpret_cast<uintptr_t>(dy) & 15) == 0,
                    "colsum: N=%d / ld=%lld must be multiples of %d and the base 16B aligned", N, ld, vec);
-  const int col_blocks = (N / vec + 31) / 32;
-  int row_blocks = max(1, min((M + 63) / 64, (num_sms() * 8 + col_blocks - 1) / col_blocks));
-  const int rows_per_block = (M + row_blocks - 1) / row_blocks;
-  row_blocks = (M + rows_per_block - 1) / rows_per_block;
-  dim3 grid(col_blocks, row_blocks);
+  int row_blocks, rows_per_block;
+  colsum_grid(M, N, vec, part ? DET_SMS : num_sms(), row_blocks, rows_per_block);
+  dim3 grid((N / vec + 31) / 32, row_blocks);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (dy_is_fp32) colsum_kernel<true><<<grid, 256, 0, st>>>(dy, ld, out, M, N, rows_per_block);
-  else colsum_kernel<false><<<grid, 256, 0, st>>>(dy, ld, out, M, N, rows_per_block);
+  if (dy_is_fp32) colsum_kernel<true><<<grid, 256, 0, st>>>(dy, ld, out, M, N, rows_per_block, part);
+  else colsum_kernel<false><<<grid, 256, 0, st>>>(dy, ld, out, M, N, rows_per_block, part);
   EGOVLP_CHECK_LAUNCH();
-  return EGOVLP_OK;
+  return part ? ordered_sum(part, row_blocks, N, out, st) : EGOVLP_OK;
+}
+
+extern "C" int egovlp_colsum_accum(const void* dy, int dy_is_fp32, long long ld, float* out, int M, int N,
+                                   void* stream) {
+  return colsum_impl(dy, dy_is_fp32, ld, out, M, N, nullptr, stream);
+}
+
+extern "C" long long egovlp_colsum_det_workspace_floats(int M, int N, int dy_is_fp32) {
+  if (M < 0 || N <= 0) return -1;
+  if (M == 0) return 0;
+  int row_blocks, rows_per_block;
+  colsum_grid(M, N, dy_is_fp32 ? 4 : 8, DET_SMS, row_blocks, rows_per_block);
+  return (long long)row_blocks * N;
+}
+
+extern "C" int egovlp_colsum_accum_det(const void* dy, int dy_is_fp32, long long ld, float* out, int M, int N, float* ws,
+                                       void* stream) {
+  EGOVLP_CHECK_ARG(ws, "colsum_det: null workspace");
+  return colsum_impl(dy, dy_is_fp32, ld, out, M, N, ws, stream);
 }

@@ -171,7 +171,7 @@ __global__ void nce_bwd_kernel(const float* __restrict__ x, const uint8_t* __res
 // m_i = margin (model/loss.py:63-90) or margin * weight[i] (AdaptiveMaxMarginRankingLoss, model/loss.py:100-133: the
 // weight is expanded along the row of the anchor i in BOTH directions).
 __global__ void maxmargin_fwd_kernel(const float* __restrict__ x, const float* __restrict__ weight, int G, float margin,
-                                     int fix_norm, float* __restrict__ loss) {
+                                     int fix_norm, float* __restrict__ loss, float* __restrict__ part) {
   __shared__ float red[32];
   float s = 0.f;
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < (long long)G * G;
@@ -188,7 +188,10 @@ __global__ void maxmargin_fwd_kernel(const float* __restrict__ x, const float* _
     s = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.f;
     s = warp_sum(s);
     const float denom = fix_norm ? 2.f * G * (G - 1) : 2.f * G * G;
-    if (threadIdx.x == 0) atomicAdd(loss, s / denom);
+    if (threadIdx.x == 0) {
+      if (part) part[blockIdx.x] = s / denom;      // deterministic form: merged in CTA order
+      else atomicAdd(loss, s / denom);
+    }
   }
 }
 // dx accumulated with atomics: each (i,j) term touches x_ii, x_ij, x_ji
@@ -205,6 +208,32 @@ __global__ void maxmargin_bwd_kernel(const float* __restrict__ x, const float* _
   if (m - (d - x[idx]) > 0.f) { atomicAdd(dx + idx, g); dd -= g; }
   if (m - (d - x[(long long)j * G + i]) > 0.f) { atomicAdd(dx + (long long)j * G + i, g); dd -= g; }
   if (dd != 0.f) atomicAdd(dx + (long long)i * G + i, dd);
+}
+// Gather form of maxmargin_bwd_kernel (deterministic: each element written by one thread).  Off the diagonal, dx_ij
+// takes the term of anchor i (margin m_i against x_ij) and then the term of anchor j (margin m_j against its column
+// entry x_ij); the diagonal sums its row's terms in j order.  A pair (i, i) contributes +g +g -2g = 0 and is skipped.
+__global__ void maxmargin_bwd_gather_kernel(const float* __restrict__ x, const float* __restrict__ weight, int G,
+                                            float margin, int fix_norm, const float* __restrict__ gscale,
+                                            float* __restrict__ dx) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long long)G * G) return;
+  const int i = idx / G, j = idx % G;
+  const float denom = fix_norm ? 2.f * G * (G - 1) : 2.f * G * G;
+  const float g = (gscale ? *gscale : 1.f) / denom;
+  const float di = x[(long long)i * G + i], mi = weight ? margin * weight[i] : margin;
+  float v = 0.f;
+  if (i != j) {
+    const float dj = x[(long long)j * G + j], mj = weight ? margin * weight[j] : margin;
+    if (mi - (di - x[idx]) > 0.f) v += g;
+    if (mj - (dj - x[idx]) > 0.f) v += g;
+  } else {
+    for (int k = 0; k < G; ++k) {
+      if (k == i) continue;
+      if (mi - (di - x[(long long)i * G + k]) > 0.f) v -= g;
+      if (mi - (di - x[(long long)k * G + i]) > 0.f) v -= g;
+    }
+  }
+  dx[idx] = v;
 }
 
 // dual softmax: y = softmax(s / temp, dim=1) * s ; out = softmax(y, dim=0)
@@ -401,15 +430,28 @@ extern "C" int egovlp_nce_bwd(const float* x, const uint8_t* mask, const float* 
   EGOVLP_CHECK_LAUNCH();
   return EGOVLP_OK;
 }
-extern "C" int egovlp_maxmargin_fwd(const float* x, const float* row_weight, int G, float margin, int fix_norm,
-                                    float* loss, void* stream) {
+static int maxmargin_grid(int G) {
+  const long long n = (long long)G * G;
+  return (int)((n + 255) / 256 > 1024 ? 1024 : (n + 255) / 256);
+}
+static int maxmargin_fwd_impl(const float* x, const float* row_weight, int G, float margin, int fix_norm, float* loss,
+                              float* part, void* stream) {
   EGOVLP_CHECK_ARG(x && loss && G > 1, "maxmargin_fwd: bad args");
   EGOVLP_CHECK_CUDA(cudaMemsetAsync(loss, 0, sizeof(float), ST(stream)));
-  const long long n = (long long)G * G;
-  const int grid = (int)((n + 255) / 256 > 1024 ? 1024 : (n + 255) / 256);
-  maxmargin_fwd_kernel<<<grid, 256, 0, ST(stream)>>>(x, row_weight, G, margin, fix_norm, loss);
+  const int grid = maxmargin_grid(G);
+  maxmargin_fwd_kernel<<<grid, 256, 0, ST(stream)>>>(x, row_weight, G, margin, fix_norm, loss, part);
   EGOVLP_CHECK_LAUNCH();
-  return EGOVLP_OK;
+  return part ? ordered_sum(part, grid, 1, loss, ST(stream)) : EGOVLP_OK;
+}
+extern "C" int egovlp_maxmargin_fwd(const float* x, const float* row_weight, int G, float margin, int fix_norm,
+                                    float* loss, void* stream) {
+  return maxmargin_fwd_impl(x, row_weight, G, margin, fix_norm, loss, nullptr, stream);
+}
+extern "C" long long egovlp_maxmargin_det_workspace_floats(int G) { return G > 1 ? maxmargin_grid(G) : -1; }
+extern "C" int egovlp_maxmargin_fwd_det(const float* x, const float* row_weight, int G, float margin, int fix_norm,
+                                        float* loss, float* ws, void* stream) {
+  EGOVLP_CHECK_ARG(ws, "maxmargin_fwd_det: null workspace");
+  return maxmargin_fwd_impl(x, row_weight, G, margin, fix_norm, loss, ws, stream);
 }
 extern "C" int egovlp_maxmargin_bwd(const float* x, const float* row_weight, int G, float margin, int fix_norm,
                                     const float* gscale, float* dx, void* stream) {
@@ -417,6 +459,15 @@ extern "C" int egovlp_maxmargin_bwd(const float* x, const float* row_weight, int
   const long long n = (long long)G * G;
   EGOVLP_CHECK_CUDA(cudaMemsetAsync(dx, 0, n * sizeof(float), ST(stream)));
   maxmargin_bwd_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ST(stream)>>>(x, row_weight, G, margin, fix_norm, gscale, dx);
+  EGOVLP_CHECK_LAUNCH();
+  return EGOVLP_OK;
+}
+extern "C" int egovlp_maxmargin_bwd_det(const float* x, const float* row_weight, int G, float margin, int fix_norm,
+                                        const float* gscale, float* dx, void* stream) {
+  EGOVLP_CHECK_ARG(x && dx && G > 1, "maxmargin_bwd_det: bad args");
+  const long long n = (long long)G * G;
+  maxmargin_bwd_gather_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ST(stream)>>>(x, row_weight, G, margin, fix_norm,
+                                                                                 gscale, dx);
   EGOVLP_CHECK_LAUNCH();
   return EGOVLP_OK;
 }

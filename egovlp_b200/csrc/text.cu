@@ -30,6 +30,32 @@ __global__ void text_embed_bwd_kernel(const long long* __restrict__ ids, const f
   atomicAdd(dpos + (long long)(tok % L) * D + d, g);
 }
 
+// Deterministic form of text_embed_bwd_kernel, from the ids stably sorted (sorted[i] = ids[perm[i]], perm ascending within
+// equal ids): the CTA at the first position of each run of equal ids adds that vocabulary row's token gradients in token
+// order; dpos below sums each position over the batch in b order.  Every element is written by one thread.
+__global__ void __launch_bounds__(256)
+text_embed_bwd_word_det_kernel(const long long* __restrict__ sorted, const long long* __restrict__ perm,
+                               const float* __restrict__ dsum, float* __restrict__ dword, int ntok, int D) {
+  const int i = blockIdx.x;
+  const long long id = sorted[i];
+  if (i > 0 && sorted[i - 1] == id) return;
+  int end = i + 1;
+  while (end < ntok && sorted[end] == id) ++end;
+  for (int d = threadIdx.x; d < D; d += blockDim.x) {
+    float acc = dword[id * D + d];
+    for (int j = i; j < end; ++j) acc += dsum[perm[j] * D + d];
+    dword[id * D + d] = acc;
+  }
+}
+__global__ void text_embed_bwd_pos_det_kernel(const float* __restrict__ dsum, float* __restrict__ dpos, int B, int L,
+                                              int D) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)L * D) return;
+  float acc = dpos[i];
+  for (int b = 0; b < B; ++b) acc += dsum[(long long)b * L * D + i];
+  dpos[i] = acc;
+}
+
 // One CTA per (b, h).  qkv bf16 [B*L, 3*D] (q pre-scaled), mask int64 [B, L] (0 = padded key).
 template <bool BWD>
 __global__ void __launch_bounds__(256)
@@ -233,6 +259,16 @@ extern "C" int egovlp_text_embed_bwd(const long long* input_ids, const float* ds
   EGOVLP_CHECK_ARG(input_ids && dsum && dword && dpos && B > 0 && L > 0, "text_embed_bwd: bad args");
   const long long n = (long long)B * L * D;
   text_embed_bwd_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ST(stream)>>>(input_ids, dsum, dword, dpos, B * L, L, D);
+  EGOVLP_CHECK_LAUNCH();
+  return EGOVLP_OK;
+}
+extern "C" int egovlp_text_embed_bwd_det(const long long* sorted_ids, const long long* perm, const float* dsum,
+                                         float* dword, float* dpos, int B, int L, int D, void* stream) {
+  EGOVLP_CHECK_ARG(sorted_ids && perm && dsum && dword && dpos && B > 0 && L > 0 && D > 0, "text_embed_bwd_det: bad args");
+  text_embed_bwd_word_det_kernel<<<B * L, 256, 0, ST(stream)>>>(sorted_ids, perm, dsum, dword, B * L, D);
+  EGOVLP_CHECK_LAUNCH();
+  const long long n = (long long)L * D;
+  text_embed_bwd_pos_det_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ST(stream)>>>(dsum, dpos, B, L, D);
   EGOVLP_CHECK_LAUNCH();
   return EGOVLP_OK;
 }

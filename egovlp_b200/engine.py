@@ -46,6 +46,37 @@ class _ZeroArena:
 
 _tls = threading.local()        # per autograd thread (= per device): the arena of the block backward in progress
 
+# Under torch.use_deterministic_algorithms, torch NaN-fills every torch.empty (torch.utils.deterministic.
+# fill_uninitialized_memory).  The towers' Functions allocate their activations and gradients with torch.empty and write
+# every element with their kernels before anything reads it, so the fill is pure cost there: 29 ms of a 231 ms cfg3 step
+# on an H100.  `_library_buffers` turns it off while one of them runs.  The setting is process-wide, so a torch.empty
+# on another thread during that window is not filled either; it is restored when the last such Function returns.
+_fill_lock = threading.Lock()
+_fill_depth = 0
+_fill_saved = True
+
+
+def _library_buffers(fn):
+    @functools.wraps(fn)
+    def wrapped(*args, **kw):
+        global _fill_depth, _fill_saved
+        import torch.utils.deterministic as tud
+        if not torch.are_deterministic_algorithms_enabled():
+            return fn(*args, **kw)
+        with _fill_lock:
+            if _fill_depth == 0:
+                _fill_saved = tud.fill_uninitialized_memory
+                tud.fill_uninitialized_memory = False
+            _fill_depth += 1
+        try:
+            return fn(*args, **kw)
+        finally:
+            with _fill_lock:
+                _fill_depth -= 1
+                if _fill_depth == 0:
+                    tud.fill_uninitialized_memory = _fill_saved
+    return wrapped
+
 
 def _zeros(shape, like):
     arena = getattr(_tls, "arena", None)
@@ -269,6 +300,18 @@ def _split_for(n_out, n_in, k_rows, n_sm=132):
     num_kb = (k_rows + 63) // 64
     if os.environ.get("EGOVLP_WGRAD_SPLIT", "waves") == "legacy":       # A/B knob: the round-1 rule
         return max(1, min(num_kb, round(400 / tiles)))
+    return _waves_split(tiles, num_kb, n_sm)
+
+
+@functools.lru_cache(maxsize=None)
+def _det_split_for(n_out, n_in, k_rows):
+    """Split-K factor of a weight-gradient GEMM under torch.use_deterministic_algorithms: the waves rule of `_split_for`
+    for 132 SMs on every card, whatever EGOVLP_WGRAD_SPLIT says.  The split fixes which k-blocks each partial sums and so
+    the bits of dW: taking it from the shapes alone gives the same bits on H100 SXM (132 SMs) and PCIe (114)."""
+    return _waves_split(((n_out + 127) // 128) * ((n_in + 255) // 256), (k_rows + 63) // 64, 132)
+
+
+def _waves_split(tiles, num_kb, n_sm):
     costs = {}
     for s in range(1, min(num_kb, 64) + 1):
         kbs = -(-num_kb // s)
@@ -285,16 +328,20 @@ def wgrad(dy16, x16, n_out, n_in, bias_grad=None):
     """dW[n_out, n_in] = dy^T x (contraction over token rows), fp32, split-K atomics.  `bias_grad` (fp32 [n_out],
     zero-initialised) additionally receives colsum(dy), summed from the dy tiles while they are in shared memory."""
     dw = _zeros((n_out, n_in), dy16)
-    ops.gemm(dy16, x16, dw, a_mn=True, b_mn=True, accumulate=True, split_k=_split_for(n_out, n_in, dy16.shape[0], _sm_count(dy16.device.index)),
-             colsum_a=bias_grad)
+    if ops.deterministic():
+        split = _det_split_for(n_out, n_in, dy16.shape[0])
+    else:
+        split = _split_for(n_out, n_in, dy16.shape[0], _sm_count(dy16.device.index))
+    ops.gemm(dy16, x16, dw, a_mn=True, b_mn=True, accumulate=True, split_k=split, colsum_a=bias_grad)
     return dw
 
 
 def wgrad_and_bgrad(dy16, x16, n_out, n_in):
     """(dW, db) of a Linear from its bf16 output gradient: one GEMM when the fused column sums apply (n_in % 256 == 0;
     +1.0 % on the step, A/B on one box: 280.5 / 282.7 vs 278.5 / 278.9 clips/s; EGOVLP_WGRAD_COLSUM=0 disables), else
-    GEMM + a column-sum pass over dy."""
-    if _WGRAD_COLSUM and n_in % 256 == 0 and n_out % 8 == 0:
+    GEMM + a column-sum pass over dy.  Under torch.use_deterministic_algorithms the fused form is taken whatever
+    EGOVLP_WGRAD_COLSUM says, so that the bits of db follow from the shapes alone."""
+    if (_WGRAD_COLSUM or ops.deterministic()) and n_in % 256 == 0 and n_out % 8 == 0:
         db = _zeros((n_out,), dy16)
         return wgrad(dy16, x16, n_out, n_in, bias_grad=db), db
     return wgrad(dy16, x16, n_out, n_in), bgrad(dy16)
@@ -383,6 +430,7 @@ class PatchEmbedFn(torch.autograd.Function):
     training pos_drop (:244, 320-321) when `drop` (an ops.Drop) is given."""
 
     @staticmethod
+    @_library_buffers
     def forward(ctx, video, cls_token, pos_embed, temporal_embed, w, b, cache, norm=None, drop=None):
         B, T, C, H, W = video.shape
         D, _, P, _ = w.shape
@@ -409,6 +457,7 @@ class PatchEmbedFn(torch.autograd.Function):
         return x.view(B, S, D)
 
     @staticmethod
+    @_library_buffers
     def backward(ctx, dx):
         (patches,) = ctx.saved_tensors
         B, T, N, D, K, F = ctx.dims
@@ -494,6 +543,7 @@ class SpaceTimeBlockFn(torch.autograd.Function):
     """
 
     @staticmethod
+    @_library_buffers
     def forward(ctx, x, dims, eps, cache, *p):
         (n1w, n1b, sqw, sqb, spw, spb, tqw, tqb, tpw, tpb, n2w, n2b, f1w, f1b, f2w, f2b, n3w, n3b) = p
         B, T, N, H, grad_mode, low_memory, fp8, drop = dims
@@ -572,6 +622,7 @@ class SpaceTimeBlockFn(torch.autograd.Function):
         raise ValueError(which)
 
     @staticmethod
+    @_library_buffers
     def backward(ctx, dy):
         sv = ctx.saved_tensors
         (x2, n3, mean3, rstd3, qkv_t, a_t, lse_t, tr, n1, mean1, rstd1, qkv_s, a_s, lse_s, sr, n2, mean2, rstd2, u,
@@ -679,6 +730,7 @@ class ClsHeadFn(torch.autograd.Function):
     LayerNorm is applied to the B CLS rows only (the reference normalises all S rows, then slices)."""
 
     @staticmethod
+    @_library_buffers
     def forward(ctx, x, eps, cache, nw, nb, pw, pb):
         B, S, D = x.shape
         x = x.contiguous()
@@ -698,6 +750,7 @@ class ClsHeadFn(torch.autograd.Function):
         return out
 
     @staticmethod
+    @_library_buffers
     def backward(ctx, dout):
         B, S, D = ctx.shape
         dout = dout.contiguous().float()
@@ -939,11 +992,13 @@ class TextTowerFn(torch.autograd.Function):
     output.  (0, 0) = eval mode / the deterministic parity path."""
 
     @staticmethod
+    @_library_buffers
     def forward(ctx, input_ids, attention_mask, heads, eps, tokens_mode, cache, drop, *p):
         """`tokens_mode`: False / True, or a (tokens_mode, grad_mode) pair -- see SpaceTimeBlockFn.forward."""
         return _text_tower_fwd(ctx, False, input_ids, attention_mask, heads, eps, tokens_mode, cache, drop, p)
 
     @staticmethod
+    @_library_buffers
     def backward(ctx, dout):
         return _text_tower_bwd(ctx, dout)
 
@@ -964,10 +1019,12 @@ class BertTowerFn(torch.autograd.Function):
     1 + 2 * n + layer = attention output dense."""
 
     @staticmethod
+    @_library_buffers
     def forward(ctx, input_ids, attention_mask, heads, eps, tokens_mode, cache, drop, *p):
         return _text_tower_fwd(ctx, True, input_ids, attention_mask, heads, eps, tokens_mode, cache, drop, p)
 
     @staticmethod
+    @_library_buffers
     def backward(ctx, dout):
         return _text_tower_bwd(ctx, dout)
 

@@ -4,7 +4,7 @@ import ctypes as C
 
 import torch
 
-from ._lib import GemmEpilogue, call, lib
+from ._lib import GemmEpilogue, call, count_launches, lib
 
 BF16, F32, E4M3 = torch.bfloat16, torch.float32, torch.float8_e4m3fn
 
@@ -15,6 +15,30 @@ def _ptr(t):
 
 def _stream():
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def deterministic():
+    """torch.are_deterministic_algorithms_enabled(), read at every call as torch reads it: while it is set, every op
+    below that reduces across CTAs takes its deterministic form (partials in a workspace, merged in an order that
+    depends on the shapes only), so equal inputs give equal bits.  An op without such a form raises RuntimeError."""
+    return torch.are_deterministic_algorithms_enabled()
+
+
+_det_cache = {}       # (device index, stream) -> the fp32 workspace of the deterministic forms, grown on demand
+
+
+def _det_ws(n_floats, device):
+    """Workspace of a deterministic form: one buffer per (device, stream), grown on demand and shared by the calls on
+    that stream (stream order keeps them apart).  The kernels write every element they read back, so the buffer is
+    allocated once instead of per call: under torch's deterministic mode a fresh torch.empty is NaN-filled, which for
+    the weight gradients alone would be 9 x 9.4 MB of fill per fc1 / fc2 call."""
+    assert n_floats >= 0, "deterministic form: unsupported shape"
+    device = torch.device(device)
+    key = (device.index, torch.cuda.current_stream(device).cuda_stream)
+    buf = _det_cache.get(key)
+    if buf is None or buf.numel() < n_floats:
+        _det_cache[key] = buf = torch.empty(max(int(n_floats), 1), dtype=F32, device=device)
+    return buf
 
 
 def _chk(t, dtype, name):
@@ -68,7 +92,9 @@ def gemm(a, b, out, *, a_mn=False, b_mn=False, bias=None, residual=None, aux=Non
          drop=None):
     """out = epi(A @ B^T).  a: [M,K] (or [K,M] if a_mn), b: [N,K] (or [K,N] if b_mn); 2-D, last-dim contiguous.
     out: bf16 or fp32 [M,N]; accumulate=True -> fp32 atomic add into `out` (required for split_k>1).
-    drop: None or a `Drop`: the epilogue's dropout forms (include/egovlp_b200.h, egovlp_gemm_epilogue.drop_*)."""
+    drop: None or a `Drop`: the epilogue's dropout forms (include/egovlp_b200.h, egovlp_gemm_epilogue.drop_*).
+    Under `deterministic()`, accumulate / colsum_a take the workspace form (egovlp_gemm_epilogue.det_ws): out +=
+    P_0 + ... + P_{s-1} left to right over the splits' partial tiles."""
     _chk(a, BF16, "a"); _chk(b, BF16, "b")
     assert a.dim() == 2 and b.dim() == 2 and a.stride(1) == 1 and b.stride(1) == 1
     (K, M) = a.shape if a_mn else a.shape[::-1]
@@ -107,12 +133,23 @@ def gemm(a, b, out, *, a_mn=False, b_mn=False, bias=None, residual=None, aux=Non
     if colsum_a is not None:                 # wgrad form only: column sums of A accumulated from the smem tiles
         _chk(colsum_a, F32, "colsum_a"); assert a_mn and b_mn and colsum_a.numel() == M
     e.colsum_a = colsum_a.data_ptr() if colsum_a is not None else None
+    ws = None
+    det = deterministic()
+    if det and colsum is not None:
+        raise RuntimeError("egovlp gemm: the output column sums (colsum) have no deterministic form; "
+                           "use colsum_accum on the output instead")
+    # one split without colsum_a adds each element once: the atomic form is already deterministic
+    if det and ((accumulate and split_k > 1) or colsum_a is not None):
+        ws = _det_ws(lib().egovlp_gemm_det_workspace_floats(M, N, K, split_k), out.device)
+        e.det_ws = ws.data_ptr()
     if drop is not None:
         e.drop_p, e.drop_seed, e.drop_site = drop.p, drop.seed, drop.site
         e.path_p, e.path_site, e.path_rows = drop.path_p, drop.path_site, drop.path_rows
     with _Probe("gemm", 2.0 * M * N * K):
         call("egovlp_gemm_bf16", _ptr(a), int(a_mn), C.c_longlong(a.stride(0)), _ptr(b), int(b_mn),
              C.c_longlong(b.stride(0)), M, N, K, C.byref(e), split_k, _stream())
+    if ws is not None:              # the ordered merge passes of the deterministic form
+        count_launches(int(accumulate) + int(colsum_a is not None))
     return out
 
 
@@ -154,12 +191,16 @@ def layernorm_bwd(dy, x, gamma, mean, rstd, *, add1=None, add2=None, dx=None, dx
     assert dx16 is None or (dx16.dtype == BF16 and dx16.is_contiguous() and dx16.shape == (rows, D))
     nbytes = rows * D * (dy.element_size() + 4 + sum(t.element_size() for t in (add1, add2) if t is not None)
                          + 4 * (dx is not None) + 2 * (dx16 is not None))
+    args = (_ptr(dy), int(dy.dtype == BF16), C.c_longlong(dy.stride(0)), _ptr(x), C.c_longlong(x.stride(0)),
+            _ptr(gamma), _ptr(mean), _ptr(rstd), _ptr(add1), int(add1 is not None and add1.dtype == BF16), _ptr(add2),
+            int(add2 is not None and add2.dtype == BF16), _ptr(dx), C.c_longlong(dx.stride(0) if dx is not None else D),
+            _ptr(dx16), _ptr(dgamma), _ptr(dbeta), _ptr(colsum_dx), rows, D)
     with _Probe("layernorm_bwd", nbytes):
-        call("egovlp_layernorm_bwd", _ptr(dy), int(dy.dtype == BF16), C.c_longlong(dy.stride(0)), _ptr(x),
-             C.c_longlong(x.stride(0)), _ptr(gamma), _ptr(mean), _ptr(rstd), _ptr(add1),
-             int(add1 is not None and add1.dtype == BF16), _ptr(add2), int(add2 is not None and add2.dtype == BF16),
-             _ptr(dx), C.c_longlong(dx.stride(0) if dx is not None else D), _ptr(dx16), _ptr(dgamma), _ptr(dbeta),
-             _ptr(colsum_dx), rows, D, _stream())
+        if deterministic() and (dgamma is not None or dbeta is not None or colsum_dx is not None):
+            ws = _det_ws(lib().egovlp_layernorm_bwd_det_workspace_floats(rows, D), x.device)
+            call("egovlp_layernorm_bwd_det", *args, _ptr(ws), _stream())
+        else:
+            call("egovlp_layernorm_bwd", *args, _stream())
 
 
 def gemm_e4m3(a8, a_scale, b8, b_scale, out, *, bias=None, act=0, alpha=1.0, col_scale=1.0, col_scale_ncols=0):
@@ -235,8 +276,12 @@ def cast_multi(raw, chunk_tensor, chunk_offset):
 def colsum_accum(dy, out):
     """out[n] += sum_m dy[m,n]; dy bf16/fp32 [M,N]."""
     assert dy.dim() == 2 and dy.stride(1) == 1 and out.dtype == F32 and out.numel() == dy.shape[1]
-    call("egovlp_colsum_accum", _ptr(dy), int(dy.dtype == F32), C.c_longlong(dy.stride(0)), _ptr(out), dy.shape[0],
-         dy.shape[1], _stream())
+    args = (_ptr(dy), int(dy.dtype == F32), C.c_longlong(dy.stride(0)), _ptr(out), dy.shape[0], dy.shape[1])
+    if deterministic():
+        ws = _det_ws(lib().egovlp_colsum_det_workspace_floats(dy.shape[0], dy.shape[1], int(dy.dtype == F32)), dy.device)
+        call("egovlp_colsum_accum_det", *args, _ptr(ws), _stream())
+    else:
+        call("egovlp_colsum_accum", *args, _stream())
 
 
 def divided_attn_fwd(qkv, B, T, N, H, mode):
@@ -260,12 +305,16 @@ def divided_attn_bwd(qkv, out, dout, lse, B, T, N, H, mode, q_scale, dqkv=None):
     assert qkv.is_contiguous() and out.is_contiguous() and dout.is_contiguous() and lse.is_contiguous()
     if dqkv is None:
         dqkv = torch.empty_like(qkv)
-    ws = torch.empty(B * H * 3 * 64, dtype=F32, device=qkv.device)
+    det = deterministic()
+    if det:      # one CLS-row slot per group (and part), summed in order
+        ws = _det_ws(lib().egovlp_divided_attn_bwd_det_workspace_floats(B, T, N, H, mode), qkv.device)
+    else:
+        ws = torch.empty(B * H * 3 * 64, dtype=F32, device=qkv.device)
     S, D = 1 + T * N, 64 * H
     # algorithmic bytes: read q|k|v, out, dout and the lse once, write dq|dk|dv
     with _Probe("attn_time_bwd" if mode == 0 else "attn_space_bwd", B * S * (16 * D + 4 * H)):
-        call("egovlp_divided_attn_bwd", _ptr(qkv), _ptr(out), _ptr(dout), _ptr(lse), _ptr(dqkv), _ptr(ws), B, T, N, H,
-             mode, C.c_float(q_scale), _stream())
+        call("egovlp_divided_attn_bwd_det" if det else "egovlp_divided_attn_bwd", _ptr(qkv), _ptr(out), _ptr(dout),
+             _ptr(lse), _ptr(dqkv), _ptr(ws), B, T, N, H, mode, C.c_float(q_scale), _stream())
     return dqkv
 
 
@@ -378,6 +427,11 @@ def video_pos_table(cls_token, pos_embed, temporal_embed, conv_bias, table, T, N
 
 
 def video_embed_bwd(dx, tmp, dcls, dpos, dtemporal, dbias, B, T, N, D):
+    if deterministic():
+        ws = _det_ws(T * D, dx.device)
+        call("egovlp_video_embed_bwd_det", _ptr(dx), _ptr(tmp), _ptr(dcls), _ptr(dpos), _ptr(dtemporal), _ptr(dbias),
+             _ptr(ws), B, T, N, D, _stream())
+        return
     call("egovlp_video_embed_bwd", _ptr(dx), _ptr(tmp), _ptr(dcls), _ptr(dpos), _ptr(dtemporal), _ptr(dbias), B, T, N,
          D, _stream())
 
@@ -389,6 +443,12 @@ def text_embed_fwd(ids, word, pos, out, B, L, D):
 
 
 def text_embed_bwd(ids, dsum, dword, dpos, B, L, D):
+    if deterministic():
+        # a stable sort groups each vocabulary row's tokens, in token order (int64 plumbing, deterministic in torch)
+        sorted_ids, perm = torch.sort(ids.reshape(-1), stable=True)
+        call("egovlp_text_embed_bwd_det", _ptr(sorted_ids), _ptr(perm), _ptr(dsum), _ptr(dword), _ptr(dpos), B, L, D,
+             _stream())
+        return
     call("egovlp_text_embed_bwd", _ptr(ids), _ptr(dsum), _ptr(dword), _ptr(dpos), B, L, D, _stream())
 
 
@@ -671,6 +731,11 @@ def maxmargin_fwd(x, margin, fix_norm, row_weight=None):
         _chk(row_weight, F32, "row_weight")
         assert row_weight.shape == (x.shape[0],) and row_weight.is_contiguous()
     loss = torch.empty((), dtype=F32, device=x.device)
+    if deterministic():
+        ws = _det_ws(lib().egovlp_maxmargin_det_workspace_floats(x.shape[0]), x.device)
+        call("egovlp_maxmargin_fwd_det", _ptr(x), _ptr(row_weight), x.shape[0], C.c_float(margin), int(fix_norm),
+             _ptr(loss), _ptr(ws), _stream())
+        return loss
     call("egovlp_maxmargin_fwd", _ptr(x), _ptr(row_weight), x.shape[0], C.c_float(margin), int(fix_norm), _ptr(loss),
          _stream())
     return loss
@@ -678,7 +743,7 @@ def maxmargin_fwd(x, margin, fix_norm, row_weight=None):
 
 def maxmargin_bwd(x, margin, fix_norm, gscale, row_weight=None):
     dx = torch.empty_like(x)
-    call("egovlp_maxmargin_bwd", _ptr(x), _ptr(row_weight), x.shape[0], C.c_float(margin), int(fix_norm), _ptr(gscale),
+    call("egovlp_maxmargin_bwd_det" if deterministic() else "egovlp_maxmargin_bwd", _ptr(x), _ptr(row_weight), x.shape[0], C.c_float(margin), int(fix_norm), _ptr(gscale),
          _ptr(dx), _stream())
     return dx
 

@@ -86,10 +86,21 @@ typedef struct egovlp_gemm_epilogue {
   float path_p;
   unsigned int path_site;
   int path_rows;
+  /* Deterministic form (NULL: off), for out_mode 2 and / or colsum_a: an fp32 workspace of
+   * egovlp_gemm_det_workspace_floats(M, N, K, split_k) floats, 16B aligned.  Each split s stores its partial tile P_s
+   * (the products of its k-blocks, times alpha) to the workspace, and an ordered pass then computes
+   * out = ((out + P_0) + P_1) + ... + P_{s-1} in fp32; colsum_a gets the same treatment, its per-split partial being
+   * the sum of its n-block partials in n-block order (a split's k-blocks are shared among the n-blocks counting from
+   * the split's first).  The result depends on the operands, M, N, K and split_k only: a split's partial equals the
+   * output of a one-split GEMM over that split's rows of A and B.  Not with colsum (EGOVLP_ERR_ARG). */
+  float* det_ws;
 } egovlp_gemm_epilogue;
 
 int egovlp_gemm_bf16(const void* A, int a_mn_major, long long lda, const void* B, int b_mn_major, long long ldb,
                      int M, int N, int K, const egovlp_gemm_epilogue* epi, int split_k, void* stream);
+/* Workspace of the deterministic form: splits' * Mp * N + splits' * nb * Mp floats, splits' = the split count after
+ * empty splits are dropped, Mp = M rounded up to 128, nb = N / 256 when N % 256 == 0, else ceil(N / 128). */
+long long egovlp_gemm_det_workspace_floats(int M, int N, int K, int split_k);
 /* e4m3 inference form of the same GEMM (the video tower's LayerNorm-fed qkv and Mlp.fc1 GEMMs, opt-in,
  * SpaceTimeTransformer.set_inference_precision("fp8")):
  *   D[m,n] = epi( (sum_k A8[m,k] * B8[n,k]) * row_scale[m] * col_scale[n] )
@@ -127,6 +138,16 @@ int egovlp_layernorm_bwd(const void* dy, int dy_is_bf16, long long lddy, const f
                          const float* gamma, const float* mean, const float* rstd, const void* add1, int add1_is_bf16,
                          const void* add2, int add2_is_bf16, float* dx, long long lddx, void* dx_bf16, float* dgamma,
                          float* dbeta, float* colsum_dx, int rows, int D, void* stream);
+/* Deterministic form of the backward: the same outputs, with each CTA's dgamma / dbeta / colsum_dx partials stored to
+ * ws (egovlp_layernorm_bwd_det_workspace_floats(rows, D) floats) and added into the outputs in CTA order by a second
+ * kernel.  The grid is sized for 132 SMs on every card, and the kernel (so the partition, and with it the bits of the
+ * sums) is chosen from the shapes, the strides and whether dy, x, add1 and add2 are 16-byte aligned: the pipelined
+ * kernel takes rows >= 4096, D % 128 == 0, dense rows and 16-byte aligned bases; anything else the other one. */
+long long egovlp_layernorm_bwd_det_workspace_floats(int rows, int D);
+int egovlp_layernorm_bwd_det(const void* dy, int dy_is_bf16, long long lddy, const float* x, long long ldx,
+                             const float* gamma, const float* mean, const float* rstd, const void* add1, int add1_is_bf16,
+                             const void* add2, int add2_is_bf16, float* dx, long long lddx, void* dx_bf16, float* dgamma,
+                             float* dbeta, float* colsum_dx, int rows, int D, float* ws, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Divided space-time attention core of VarAttention.forward (model/video_transformer.py:104-133) and its
@@ -146,6 +167,12 @@ int egovlp_divided_attn_fwd(const void* qkv, void* out, float* lse, float* cls_p
                             int mode, void* stream);
 int egovlp_divided_attn_bwd(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv,
                             float* dcls_ws, int B, int T, int N, int H, int mode, float q_scale, void* stream);
+/* Deterministic form of the backward: every CTA stores its CLS-row dq / dk / dv into a slot of its own (dcls_ws, of
+ * egovlp_divided_attn_bwd_det_workspace_floats() floats: [B, H, groups, parts, 3, 64], parts = 4 in the T in
+ * {4, 8, 16} time kernel, else 1), summed in group, then part, order.  The kernel follows from the geometry alone. */
+long long egovlp_divided_attn_bwd_det_workspace_floats(int B, int T, int N, int H, int mode);
+int egovlp_divided_attn_bwd_det(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv,
+                                float* dcls_ws, int B, int T, int N, int H, int mode, float q_scale, void* stream);
 /* Spatial attention for large frames: egovlp_divided_attn_{fwd,bwd} with mode = 1 (model/video_transformer.py:109-130,
  * space mode), for 1 <= N <= 1024 patches per frame (the divided attention stops at N = 255; the engine uses these
  * above that).  Same qkv / out / lse / dqkv layouts and semantics; tiled on the tensor cores (bf16 mma.sync, fp32
@@ -197,6 +224,9 @@ int egovlp_video_pos_table(const float* cls_token, const float* pos_embed, const
                            const float* conv_bias, float* table, int T, int N, int D, void* stream);
 int egovlp_video_embed_bwd(const float* dx, float* tmp_SD, float* dcls, float* dpos, float* dtemporal, float* dbias,
                            int B, int T, int N, int D, void* stream);
+/* Deterministic form: the per-frame partials of dbias go to ws_TD (fp32 [T, D]) and are added in frame order. */
+int egovlp_video_embed_bwd_det(const float* dx, float* tmp_SD, float* dcls, float* dpos, float* dtemporal, float* dbias,
+                               float* ws_TD, int B, int T, int N, int D, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Text tower pieces (DistilBERT; call sites model/model.py:117-138).  ids / attention_mask are int64 as the
@@ -232,6 +262,10 @@ int egovlp_text_embed_fwd(const long long* input_ids, const float* word_emb, con
                           int L, int D, void* stream);
 int egovlp_text_embed_bwd(const long long* input_ids, const float* dsum, float* dword, float* dpos, int B, int L, int D,
                           void* stream);
+/* Deterministic form, from the ids stably sorted (sorted_ids[i] = input_ids[perm[i]], int64 [B*L], perm ascending among
+ * equal ids): each vocabulary row adds its tokens' gradients in token order, each position its batch's in b order. */
+int egovlp_text_embed_bwd_det(const long long* sorted_ids, const long long* perm, const float* dsum, float* dword,
+                              float* dpos, int B, int L, int D, void* stream);
 int egovlp_text_attn_fwd(const void* qkv, const long long* attention_mask, void* out, int B, int L, int H, float p_drop,
                          unsigned long long seed, unsigned int site, void* stream);
 int egovlp_text_attn_bwd(const void* qkv, const long long* attention_mask, const void* dout, void* dqkv, int B, int L,
@@ -311,6 +345,14 @@ int egovlp_maxmargin_fwd(const float* x, const float* row_weight, int G, float m
                          void* stream);
 int egovlp_maxmargin_bwd(const float* x, const float* row_weight, int G, float margin, int fix_norm,
                          const float* gscale, float* dx, void* stream);
+/* Deterministic forms: the forward merges its per-CTA partials (ws: egovlp_maxmargin_det_workspace_floats(G) floats)
+ * in CTA order; the backward writes each dx element from one thread (off the diagonal: anchor i's term, then anchor
+ * j's; on it: the row's terms in j order). */
+long long egovlp_maxmargin_det_workspace_floats(int G);
+int egovlp_maxmargin_fwd_det(const float* x, const float* row_weight, int G, float margin, int fix_norm, float* loss,
+                             float* ws, void* stream);
+int egovlp_maxmargin_bwd_det(const float* x, const float* row_weight, int G, float margin, int fix_norm,
+                             const float* gscale, float* dx, void* stream);
 int egovlp_dual_softmax(const float* sim, float* out, int rows, int cols, float temp, void* stream);
 
 /* EgoNCE from the gathered embeddings, ONE kernel per direction (trainer/trainer_egoclip.py:130-135 = sim_matrix x3 +
@@ -402,6 +444,11 @@ int egovlp_cast_f32_to_bf16(const float* src, void* dst_bf16, long long n, void*
 int egovlp_quantize_rows_e4m3(const float* w, long long ldw, uint8_t* q, float* scale, int rows, int K, void* stream);
 /* out[n] += sum_m dy[m, n]  (bias gradients).  dy bf16 or fp32 [M, N] row stride ld. */
 int egovlp_colsum_accum(const void* dy, int dy_is_fp32, long long ld, float* out, int M, int N, void* stream);
+/* Deterministic form: row-block partials (ws: egovlp_colsum_det_workspace_floats(M, N, dy_is_fp32) floats, the split
+ * sized for 132 SMs on every card) added into out in row-block order. */
+long long egovlp_colsum_det_workspace_floats(int M, int N, int dy_is_fp32);
+int egovlp_colsum_accum_det(const void* dy, int dy_is_fp32, long long ld, float* out, int M, int N, float* ws,
+                            void* stream);
 /* Backward of a GEMM dropout form (egovlp_gemm_epilogue.drop_*): y bf16 [rows, W] = bf16(x[r, c] * keep(r, c) /
  * (1 - p) * f(r / path_rows)), keep and f drawn exactly as that form draws them for a [rows, W] output (f = 1 when
  * path_rows = 0): the gradient of the video tower's dropped branches (model/video_transformer.py:36-52, 135-136,
