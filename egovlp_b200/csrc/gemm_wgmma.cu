@@ -1101,6 +1101,14 @@ extern "C" int egovlp_gemm_bf16(const void* A, int a_mn_major, long long lda, co
   EGOVLP_CHECK_ARG((e->act != 2 && e->act != 4 && e->act != 5) || e->aux, "gemm: act=2/4/5 needs aux");
   EGOVLP_CHECK_ARG(e->act != 5 || e->out2, "gemm: act=5 needs out2");
   EGOVLP_CHECK_ARG(e->ldo % 8 == 0, "gemm: ldo must be a multiple of 8");
+  // the generic epilogue moves bias / residual / fp32 out / colsum as float2 and aux / bf16 out / out2 as bf16x2
+  const auto off = [](const void* p, uintptr_t align) { return (reinterpret_cast<uintptr_t>(p) & (align - 1)) != 0; };
+  EGOVLP_CHECK_ARG(!off(e->bias, 8) && !off(e->residual, 8) && !off(e->colsum, 8) && (e->out_mode == 0 || !off(e->out, 8)),
+                   "gemm: bias, residual, colsum and an fp32 out must be 8-byte aligned");
+  EGOVLP_CHECK_ARG(!off(e->aux, 4) && !off(e->out2, 4) && (e->out_mode != 0 || !off(e->out, 4)),
+                   "gemm: aux, out2 and a bf16 out must be 4-byte aligned");
+  EGOVLP_CHECK_ARG((!e->residual || e->ldr % 2 == 0) && (!e->aux || e->ldaux % 2 == 0) && (!e->out2 || e->ldo2 % 2 == 0),
+                   "gemm: ldr, ldaux and ldo2 must be even");
   EpiParams ep;
   ep.bias = e->bias; ep.residual = e->residual; ep.aux = reinterpret_cast<const bf16*>(e->aux);
   ep.out = e->out; ep.out2 = reinterpret_cast<bf16*>(e->out2);

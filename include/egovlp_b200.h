@@ -48,7 +48,8 @@ int egovlp_abi_version(void);
  *          (1 with out2 + 5 = the low-memory Mlp pair: fc1 saves the pre-activation z, and the fc2 input-gradient GEMM
  *          also rebuilds gelu(z), the fc2 weight gradient's operand);   v += residual[m,n] (fp32);
  *   out_mode 0: out(bf16) = v;  1: out(fp32) = v;  2: atomicAdd(out(fp32), v) (needed for split_k>1)
- * Constraints: N % 32 == 0, lda/ldb/ldo % 8 == 0, 16B-aligned bases.
+ * Constraints: N % 32 == 0, lda/ldb/ldo % 8 == 0, ldr/ldaux/ldo2 even; A and B 16B-aligned, bias / residual / colsum /
+ * an fp32 out 8B-aligned, aux / out2 / a bf16 out 4B-aligned (EGOVLP_ERR_ARG otherwise).
  * The library chooses the kernel instance itself (tile scheduler, compile-time specialised epilogue for the common
  * descriptor forms); every instance computes the arithmetic above in the same order, so the choice never changes a bit of
  * the result (tests/test_kernels_gpu.py::test_gemm_specialised_epilogues_match_the_generic_one).

@@ -17,6 +17,7 @@ Not tested: attention masks with no valid key at all.  The tokenizer always emit
 the kernel returns NaN (0 / 0 in the softmax), as the masked_fill(-inf) softmax of the reference does."""
 import pytest
 import torch
+from gemm_ref import check, reference
 from kernel_checks import (BF16, F32, F64, assert_bf16_ulps, assert_bits_equal, assert_rows_close, assert_sum_bound, mk,
                            nan_filled, rel_l2)
 
@@ -128,6 +129,7 @@ def test_patch_embed_gemm_adds_the_table_row_m_mod_s(ops, gemm_mode, B, S):
     print(f"[bound] patch-embedding GEMM S={S} {gemm_mode}: rel-L2 {err:.3g} (bound 2e-5)")
     assert err < 2e-5
     assert_rows_close(f"patch-embedding GEMM S={S} {gemm_mode} per row", out, ref, rtol=1e-4, atol=0.0)
+    check(f"patch-embedding GEMM S={S} {gemm_mode}", out, reference(a, w, bias=bias, residual=table, res_row_mod=S)["out"])
 
 
 @pytest.mark.parametrize("H,W,P", [(32, 48, 16), (36, 48, 12)])

@@ -4,6 +4,7 @@ memory with a TMA reduce (EPI_RED_F32).  These tests cover what that path has to
 fused bias gradient, dW views inside wider buffers, and dW tensors TMA cannot address, which take the generic epilogue."""
 import pytest
 import torch
+from gemm_ref import check, check_all, reference
 
 pytestmark = pytest.mark.gpu
 
@@ -43,11 +44,16 @@ def test_wgrad_matches_fp64(ops, tokens, n_out, n_in, split, base):
     dw = b0.clone()
     ops.gemm(dy, x, dw, a_mn=True, b_mn=True, accumulate=True, split_k=split)
     assert rel_err(dw, ref) < 2e-5
+    name = f"wgrad {(tokens, n_out, n_in, split)} {base}"
+    check(name, dw, reference(dy, x, a_mn=True, b_mn=True, base=b0, split_k=split)["out"])
     if n_in % 256 == 0:       # the fused bias gradient (column sums of dy) beside the reduce epilogue
         dw2, db = b0.clone(), torch.full((n_out,), 0.5, device="cuda")
         ops.gemm(dy, x, dw2, a_mn=True, b_mn=True, accumulate=True, split_k=split, colsum_a=db)
         assert rel_err(dw2, ref) < 2e-5
         assert rel_err(db, 0.5 + dy.double().sum(0)) < 1e-5
+        check_all(name + " + colsum_a", {"out": dw2, "colsum_a": db},
+                  reference(dy, x, a_mn=True, b_mn=True, base=b0, split_k=split,
+                            colsum_a=torch.full((n_out,), 0.5, device="cuda")))
 
 
 @pytest.mark.parametrize("tokens,n_out,n_in", [(3144, 2304, 768), (1000, 200, 96), (784, 128, 64), (2056, 768, 3072)])
@@ -64,6 +70,8 @@ def test_wgrad_single_split_is_bitwise_the_generic_epilogue(ops, monkeypatch, to
         outs.append(dw)
     torch.cuda.synchronize()
     assert torch.equal(outs[0], outs[1])
+    check(f"wgrad one split {(tokens, n_out, n_in)} {base}", outs[1],
+          reference(dy, x, a_mn=True, b_mn=True, base=b0)["out"])
 
 
 @pytest.mark.parametrize("n_out,n_in,split", [(200, 96, 3), (776, 256, 4), (136, 768, 2)])
@@ -75,6 +83,8 @@ def test_wgrad_into_a_view_leaves_the_rest_of_the_buffer(ops, n_out, n_in, split
     dw.zero_()
     ops.gemm(dy, x, dw, a_mn=True, b_mn=True, accumulate=True, split_k=split)
     assert rel_err(dw, dy.double().t() @ x.double()) < 2e-5
+    check(f"wgrad view {(n_out, n_in, split)}", dw,
+          reference(dy, x, a_mn=True, b_mn=True, base=torch.zeros_like(dw), split_k=split)["out"])
     outside = torch.ones_like(buf, dtype=torch.bool)
     outside[24:24 + n_out, 32:32 + n_in] = False
     assert buf[outside].isnan().all()
@@ -92,3 +102,5 @@ def test_wgrad_dw_tma_cannot_address_takes_the_generic_epilogue(ops, n_out, n_in
     dw.copy_(b0)
     ops.gemm(dy, x, dw, a_mn=True, b_mn=True, accumulate=True, split_k=split)
     assert rel_err(dw, b0.double() + dy.double().t() @ x.double()) < 2e-5
+    check(f"wgrad TMA-unaddressable {(n_out, n_in, split)}", dw,
+          reference(dy, x, a_mn=True, b_mn=True, base=b0, split_k=split)["out"])

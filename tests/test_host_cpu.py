@@ -34,6 +34,31 @@ def test_argument_errors_are_reported_not_swallowed():
     assert _lib.lib().egovlp_divided_attn_workspace_floats(2, 400, 196, 12, 0) == -1     # unsupported geometry
 
 
+@pytest.mark.parametrize("field,value,msg", [
+    ("bias", 0x40004, "8-byte aligned"), ("residual", 0x50004, "8-byte aligned"), ("colsum", 0x60004, "8-byte aligned"),
+    ("out", 0x30004, "8-byte aligned"),                        # fp32 out (out_mode 1)
+    ("aux", 0x70002, "4-byte aligned"), ("out2", 0x80002, "4-byte aligned"), ("out", 0x30002, "4-byte aligned"),
+    ("ldr", 769, "even"), ("ldaux", 769, "even"), ("ldo2", 769, "even")])
+def test_gemm_refuses_misaligned_epilogue_tensors(field, value, msg):
+    """The generic epilogue moves bias / residual / fp32 out / colsum as float2 and aux / bf16 out / out2 as bf16x2:
+    egovlp_gemm_bf16 must refuse a base or row stride that would misalign them, before any launch.  The addresses are
+    made up, so this runs only where no GPU could be reached by a check that failed to refuse."""
+    if torch.cuda.is_available():
+        pytest.skip("made-up device addresses: not passed where a GPU is visible")
+    import ctypes as C
+    from egovlp_b200 import _lib
+    M, N, K = 256, 768, 768
+    e = _lib.GemmEpilogue()
+    e.bias, e.residual, e.aux, e.out, e.out2 = 0x40000, 0x50000, 0x70000, 0x30000, 0x80000
+    e.ldr = e.ldaux = e.ldo = e.ldo2 = N
+    e.act, e.alpha, e.col_scale = 5, 1.0, 1.0                  # act 5 reads aux and writes out2
+    e.out_mode = 1 if (field, msg) == ("out", "8-byte aligned") else 0
+    setattr(e, field, value)
+    with pytest.raises(_lib.EgovlpError, match=msg):
+        _lib.call("egovlp_gemm_bf16", C.c_void_p(0x10000), 0, C.c_longlong(K), C.c_void_p(0x20000), 0,
+                  C.c_longlong(K), M, N, K, C.byref(e), 1, None)
+
+
 def test_state_dict_contract_matches_reference_keys():
     from egovlp_b200 import synthetic as syn
     from egovlp_b200.model.model import FrozenInTime

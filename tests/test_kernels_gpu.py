@@ -1,9 +1,12 @@
 """Per-kernel parity on the GPU: every CUDA op against a plain torch fp32 restatement of the same op
 (called through the C-ABI via egovlp_b200.ops).  The divided attention is checked against the fp64 reference of
-test_divided_attention_gpu.py (divided_attention_ref.py), element by element."""
+test_divided_attention_gpu.py (divided_attention_ref.py), element by element, and every GEMM output against the fp64
+reference and bound of gemm_ref.py, element by element, beside the relative-L2 checks."""
 import pytest
 import torch
 from divided_attention_ref import check_case
+from gemm_ref import check, check_all, gelu_tail_inputs, reference, spread
+from kernel_checks import nan_filled
 
 pytestmark = pytest.mark.gpu
 
@@ -31,27 +34,42 @@ def mk(shape, seed, scale=1.0, dtype=torch.bfloat16):
     return (torch.randn(shape, generator=g, device="cuda") * scale).to(dtype)
 
 
+def past_k(x, ld=64):
+    """x as the first columns of a [rows, ld] buffer whose other columns hold 1e4: a read past K cannot hide."""
+    buf = torch.full((x.shape[0], ld), 1e4, device="cuda", dtype=x.dtype)
+    buf[:, :x.shape[1]] = x
+    return buf[:, :x.shape[1]]
+
+
+# K = 8 and 40: one partial k-block; K = 20: a view with row stride 64 (K itself is not a multiple of 8)
 @pytest.mark.parametrize("M,N,K", [(128, 256, 64), (256, 512, 768), (300, 768, 768), (1570, 2304, 768),
-                                   (130, 128, 64), (200, 64, 128), (1000, 3072, 768), (257, 768, 3072), (64, 32, 64)])
+                                   (130, 128, 64), (200, 64, 128), (1000, 3072, 768), (257, 768, 3072), (64, 32, 64),
+                                   (300, 256, 8), (200, 384, 40), (130, 512, 20)])
 def test_gemm_kmajor_bias(ops, M, N, K, gemm_mode):
     a, b = mk((M, K), 1), mk((N, K), 2, 0.05)
+    if K % 8:
+        a, b = past_k(a), past_k(b)
     bias = mk((N,), 3, dtype=torch.float32)
-    out = torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
+    want = reference(a, b, bias=bias)["out"]
+    out = nan_filled((M, N), torch.bfloat16)
     ops.gemm(a, b, out, bias=bias)
     ref = a.float() @ b.float().t() + bias
     assert rel_err(out, ref) < 4e-3
-    out32 = torch.empty(M, N, device="cuda", dtype=torch.float32)
+    check(f"gemm bias bf16 {(M, N, K)} {gemm_mode}", out, want)
+    out32 = nan_filled((M, N), torch.float32)
     ops.gemm(a, b, out32, bias=bias)
     assert rel_err(out32, ref) < 2e-5
+    check(f"gemm bias fp32 {(M, N, K)} {gemm_mode}", out32, want)
 
 
 @pytest.mark.parametrize("M,N,K", [(256, 256, 128), (300, 768, 2304), (1000, 3072, 768), (200, 64, 128)])
 def test_gemm_b_mn_major_dgrad(ops, M, N, K, gemm_mode):
     """dx = dy @ W with W stored [K, N] (n contiguous): the dgrad form."""
     a, w = mk((M, K), 4), mk((K, N), 5, 0.05)
-    out = torch.empty(M, N, device="cuda", dtype=torch.float32)
+    out = nan_filled((M, N), torch.float32)
     ops.gemm(a, w, out, b_mn=True)
     assert rel_err(out, a.float() @ w.float()) < 2e-5
+    check(f"gemm dgrad fp32 {(M, N, K)} {gemm_mode}", out, reference(a, w, b_mn=True)["out"])
 
 
 @pytest.mark.parametrize("Mtok,N,Kin,split", [(512, 256, 256, 1), (1000, 768, 768, 4), (3137, 2304, 768, 7),
@@ -66,85 +84,121 @@ def test_gemm_both_mn_major_wgrad(ops, Mtok, N, Kin, split, gemm_mode):
     ops.gemm(dy, x, out, a_mn=True, b_mn=True, accumulate=True, split_k=split)
     ref = base + dy.float().t() @ x.float()
     assert rel_err(out, ref) < 2e-5
+    name = f"gemm wgrad {(Mtok, N, Kin, split)} {gemm_mode}"
+    check(name, out, reference(dy, x, a_mn=True, b_mn=True, base=base, split_k=split)["out"])
     if Kin % 256 == 0:        # fused bias gradient: column sums of dy taken from the smem tiles of the same GEMM
         out2, db = base.clone(), torch.full((N,), 0.5, device="cuda")
+        db0 = db.clone()
         ops.gemm(dy, x, out2, a_mn=True, b_mn=True, accumulate=True, split_k=split, colsum_a=db)
         assert rel_err(out2, ref) < 2e-5
         assert rel_err(db, 0.5 + dy.float().sum(0)) < 1e-5
+        check_all(name + " + colsum_a", {"out": out2, "colsum_a": db},
+                  reference(dy, x, a_mn=True, b_mn=True, base=base, split_k=split, colsum_a=db0))
 
 
-def test_gemm_epilogues(ops, gemm_mode):
+@pytest.mark.parametrize("inputs", ["randn", "tails"])
+def test_gemm_epilogues(ops, gemm_mode, inputs):
+    """Every epilogue of the generic form and the forms beside it, each output element-wise against fp64.  "tails": rows
+    of A scaled so that the pre-activations reach about +-10 with exact zeros among them, and an aux uniform in
+    [-10, 10] with zeros, so that GELU and GELU' are checked where few elements of random inputs lie."""
     M, N, K = 515, 768, 256
     a, b = mk((M, K), 9), mk((N, K), 10, 0.06)
     bias = mk((N,), 11, dtype=torch.float32)
     res = mk((M, N), 12, dtype=torch.float32)
+    aux = mk((M, N), 13)
+    if inputs == "tails":
+        a, bias = gelu_tail_inputs(a, bias)
+        aux = spread((M, N), 13)
+    name = f"gemm epilogue {inputs} {gemm_mode}"
     acc = a.float() @ b.float().t() + bias
     # bias + residual -> fp32
-    out = torch.empty(M, N, device="cuda", dtype=torch.float32)
+    out = nan_filled((M, N), torch.float32)
     ops.gemm(a, b, out, bias=bias, residual=res)
     assert rel_err(out, acc + res) < 2e-5
+    check(f"{name} residual fp32", out, reference(a, b, bias=bias, residual=res)["out"])
     # bias + gelu, pre-activation saved
-    h = torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
-    u = torch.empty_like(h)
+    h = nan_filled((M, N), torch.bfloat16)
+    u = nan_filled((M, N), torch.bfloat16)
     ops.gemm(a, b, h, bias=bias, act=1, out2=u)
     assert rel_err(u, acc) < 4e-3
     assert rel_err(h, torch.nn.functional.gelu(acc)) < 4e-3
+    check_all(f"{name} act 1", {"out": h, "out2": u}, reference(a, b, bias=bias, act=1, out2=True))
     # multiply by gelu'(aux)
-    aux = mk((M, N), 13)
-    out = torch.empty(M, N, device="cuda", dtype=torch.float32)
+    out = nan_filled((M, N), torch.float32)
     ops.gemm(a, b, out, aux=aux, act=2)
     x = aux.float().requires_grad_(True)
     torch.nn.functional.gelu(x).sum().backward()
     assert rel_err(out, (a.float() @ b.float().t()) * x.grad) < 1e-4
+    check(f"{name} act 2 fp32", out, reference(a, b, aux=aux, act=2)["out"])
     # same, bf16 output + fused column sums (the fc1 bias gradient)
-    out16 = torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
+    out16 = nan_filled((M, N), torch.bfloat16)
     cs = torch.ones(N, device="cuda")
     ops.gemm(a, b, out16, aux=aux, act=2, colsum=cs)
     assert rel_err(out16, out) < 4e-3
     assert rel_err(cs, 1 + out.sum(0)) < 1e-4
+    check_all(f"{name} act 2 bf16", {"out": out16, "colsum": cs},
+              reference(a, b, aux=aux, act=2, colsum=torch.ones(N, device="cuda")))
     # the Mlp pair of the training step: act 3 = GELU with its derivative saved to out2, act 4 = multiply by aux
-    h3, d3 = torch.empty_like(h), torch.empty_like(h)
+    h3, d3 = nan_filled((M, N), torch.bfloat16), nan_filled((M, N), torch.bfloat16)
     ops.gemm(a, b, h3, bias=bias, act=3, out2=d3)
     accg = acc.clone().requires_grad_(True)
     torch.nn.functional.gelu(accg).sum().backward()
     assert torch.equal(h3, h)
     assert rel_err(d3, accg.grad) < 4e-3
-    out4 = torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
+    check_all(f"{name} act 3", {"out": h3, "out2": d3}, reference(a, b, bias=bias, act=3, out2=True))
+    out4 = nan_filled((M, N), torch.bfloat16)
     cs4 = torch.ones(N, device="cuda")
     ops.gemm(a, b, out4, aux=d3, act=4, colsum=cs4)
     ref4 = (a.float() @ b.float().t()) * d3.float()
     assert rel_err(out4, ref4) < 4e-3 and rel_err(cs4, 1 + ref4.sum(0)) < 1e-4
+    check_all(f"{name} act 4", {"out": out4, "colsum": cs4},
+              reference(a, b, aux=d3, act=4, colsum=torch.ones(N, device="cuda")))
     # q-scale on the first 256 columns
-    out = torch.empty(M, N, device="cuda", dtype=torch.float32)
+    out = nan_filled((M, N), torch.float32)
     ops.gemm(a, b, out, bias=bias, col_scale=0.125, col_scale_ncols=256)
     ref = acc.clone(); ref[:, :256] *= 0.125
     assert rel_err(out, ref) < 2e-5
+    check(f"{name} column scale fp32", out, reference(a, b, bias=bias, col_scale=0.125, col_scale_ncols=256)["out"])
 
 
-@pytest.mark.parametrize("M,N,K", [(1570, 768, 256), (515, 3072, 768), (4099, 1024, 128)])
-def test_gemm_specialised_epilogues_match_the_generic_one(ops, monkeypatch, M, N, K):
+# the training step's shapes at M = 2 x 3137 and 6 x 3137 tokens (qkv, fc1, fc2 forward and fc1 dgrad), and a 128-column
+# one: at least 3 tiles per CTA (per CTA pair when pairs run), so that the bias row, the epilogue buffers and the stage
+# ring are reused across tiles with their phase bits flipping
+STEP_SHAPES = [(6274, 2304, 768), (6274, 3072, 768), (18822, 768, 3072), (17000, 384, 256)]
+
+
+@pytest.mark.parametrize("M,N,K", [(1570, 768, 256), (515, 3072, 768), (4099, 1024, 128)] + STEP_SHAPES)
+def test_gemm_specialised_epilogues_match_the_generic_one(ops, monkeypatch, gemm_mode, M, N, K):
     """The K-major-A kernels carry compile-time specialised epilogues for the step's hot forms (bias -> bf16, GELU + GELU',
     x aux, bias + fp32 residual -> fp32); EGOVLP_GEMM_GENERIC_EPI=1 routes the same calls through the generic epilogue.
-    Same arithmetic in the same order: the results must be bit-identical (ragged last m-block, several tiles per CTA)."""
+    Same arithmetic in the same order: the results must be bit-identical (ragged last m-block, several tiles per CTA),
+    and every output is held element-wise to fp64."""
+    if (M, N, K) in STEP_SHAPES:
+        pair = gemm_mode == "pair" and N % 256 == 0
+        tile_m, tile_n = (256, 256) if pair else (128, 256 if N % 256 == 0 else 128)
+        sms = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+        tiles = -(-M // tile_m) * -(-N // tile_n)
+        assert tiles >= 3 * (sms // 2 if pair else sms), (tiles, sms, pair)
     a, b = mk((M, K), 30), mk((N, K), 31, 0.06)
     wt = mk((K, N), 32, 0.06)                      # MN-major B (dgrad form)
     bias = mk((N,), 33, dtype=torch.float32)
     res = mk((M, N), 34, dtype=torch.float32)
     aux = mk((M, N), 35)
+    bf, f32 = torch.bfloat16, torch.float32
 
     def run():
         outs = []
-        o = torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
+        o = nan_filled((M, N), bf)
         ops.gemm(a, b, o, bias=bias, col_scale=0.125, col_scale_ncols=256); outs.append(o)            # EPI_BF16
-        o = torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
+        o = nan_filled((M, N), bf)
         ops.gemm(a, wt, o, b_mn=True); outs.append(o)                                                  # EPI_BF16, dgrad
-        h, d = torch.empty_like(o), torch.empty_like(o)
+        h, d = nan_filled((M, N), bf), nan_filled((M, N), bf)
         ops.gemm(a, b, h, bias=bias, act=3, out2=d); outs += [h, d]                                     # EPI_ACT3
-        o = torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
+        o = nan_filled((M, N), bf)
         ops.gemm(a, wt, o, b_mn=True, aux=aux, act=4); outs.append(o)                                   # EPI_MUL_AUX
-        o = torch.empty(M, N, device="cuda", dtype=torch.float32)
+        o = nan_filled((M, N), f32)
         ops.gemm(a, b, o, bias=bias, residual=res); outs.append(o)                                      # EPI_RES_F32
-        o = torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
+        o = nan_filled((M, N), bf)
         ops.gemm(a, b, o, bias=bias, act=1); outs.append(o)                                             # EPI_ACT1
         torch.cuda.synchronize()
         return outs
@@ -160,6 +214,14 @@ def test_gemm_specialised_epilogues_match_the_generic_one(ops, monkeypatch, M, N
     assert rel_err(got[2], torch.nn.functional.gelu(acc)) < 4e-3
     assert torch.equal(got[6], got[2])             # inference-form GELU == the training form's first output
     assert rel_err(got[4], (a.float() @ wt.float()) * aux.float()) < 4e-3
+    del acc, ref
+    name = f"gemm {(M, N, K)} {gemm_mode}"
+    check(f"{name} bf16 + column scale", got[0], reference(a, b, bias=bias, col_scale=0.125, col_scale_ncols=256)["out"])
+    check(f"{name} bf16 dgrad", got[1], reference(a, wt, b_mn=True)["out"])
+    check_all(f"{name} act 3", {"out": got[2], "out2": got[3]}, reference(a, b, bias=bias, act=3, out2=True))
+    check(f"{name} x aux dgrad", got[4], reference(a, wt, b_mn=True, aux=aux, act=4)["out"])
+    check(f"{name} residual fp32", got[5], reference(a, b, bias=bias, residual=res)["out"])
+    check(f"{name} act 1", got[6], reference(a, b, bias=bias, act=1)["out"])
 
 
 def test_gemm_strided_views(ops, gemm_mode):
@@ -170,6 +232,7 @@ def test_gemm_strided_views(ops, gemm_mode):
     ops.gemm(abuf[:, K:2 * K], bbuf[:, K:], obuf[:, N:])
     assert rel_err(obuf[:, N:], abuf[:, K:2 * K].float() @ bbuf[:, K:].float().t()) < 4e-3
     assert torch.all(obuf[:, :N] == 0)
+    check(f"gemm strided views {gemm_mode}", obuf[:, N:], reference(abuf[:, K:2 * K], bbuf[:, K:])["out"])
 
 
 @pytest.mark.parametrize("rows,D", [(1000, 768), (37, 64), (785 * 2, 768), (5, 128), (4999, 768), (6001, 128),

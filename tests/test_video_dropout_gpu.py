@@ -17,6 +17,8 @@ from functools import partial
 import pytest
 import torch
 import torch.nn.functional as F
+from gemm_ref import check, check_all, reference
+from kernel_checks import nan_filled
 from torch import nn
 
 pytestmark = pytest.mark.gpu
@@ -103,10 +105,11 @@ def test_gemm_dropout_forms_apply_the_materialised_masks(N):
 
     # proj / fc2 forward: resid + m (a w^T + b); the plain form gives the product
     plain = ops.gemm(a, w, torch.empty(M, N, device="cuda"), bias=bias, residual=torch.zeros_like(resid))
-    got = ops.gemm(a, w, torch.empty(M, N, device="cuda"), bias=bias, residual=resid, drop=d)
+    got = ops.gemm(a, w, nan_filled((M, N), torch.float32), bias=bias, residual=resid, drop=d)
     sel = plain.abs() > 1e-3                                # where the product cannot vanish into the residual's rounding
     assert torch.equal((got == resid)[sel], (m == 0)[sel])
     assert rel(got - resid, plain * m) < 1e-6
+    check(f"dropout residual fp32 N={N}", got, reference(a, w, bias=bias, residual=resid, mult=m)["out"])
 
     # fc1 forward, both training forms: h = m GELU(v); the second output is unmasked
     e = ops.Drop(0.3, 1234, 9)
@@ -114,25 +117,30 @@ def test_gemm_dropout_forms_apply_the_materialised_masks(N):
     h0, u0 = torch.empty(M, N, device="cuda", dtype=BF16), torch.empty(M, N, device="cuda", dtype=BF16)
     ops.gemm(a, w, h0, bias=bias, act=3, out2=u0)
     for act in (3, 1):
-        h, u = torch.empty_like(h0), torch.empty_like(u0)
+        h, u = nan_filled((M, N), BF16), nan_filled((M, N), BF16)
         ops.gemm(a, w, h, bias=bias, act=act, out2=u, drop=e)
         if act == 3:
             assert torch.equal(u, u0)
         assert torch.equal(h == 0, (me == 0) | (h0 == 0)) and rel(h, h0.float() * me) < 5e-3
+        check_all(f"dropout act {act} N={N}", {"out": h, "out2": u},
+                  reference(a, w, bias=bias, act=act, out2=True, mult=me))
 
     # fc2 input gradient with W2 as MN-major B: du = (dy W2) aux m;  low memory: du and h = m GELU(z)
     dy = torch.randn(M, K, device="cuda", generator=g).to(BF16)
     w2 = (0.1 * torch.randn(K, N, device="cuda", generator=g)).to(BF16)
     aux = torch.randn(M, N, device="cuda", generator=g).to(BF16)
     du0 = ops.gemm(dy, w2, torch.empty(M, N, device="cuda", dtype=BF16), b_mn=True, aux=aux, act=4)
-    du = ops.gemm(dy, w2, torch.empty(M, N, device="cuda", dtype=BF16), b_mn=True, aux=aux, act=4, drop=e)
+    du = ops.gemm(dy, w2, nan_filled((M, N), BF16), b_mn=True, aux=aux, act=4, drop=e)
     assert torch.equal(du == 0, (me == 0) | (du0 == 0)) and rel(du, du0.float() * me) < 5e-3
+    check(f"dropout act 4 N={N}", du, reference(dy, w2, b_mn=True, aux=aux, act=4, mult=me)["out"])
     du0, hz0 = torch.empty_like(du), torch.empty_like(du)
     ops.gemm(dy, w2, du0, b_mn=True, aux=aux, act=5, out2=hz0)
-    du, hz = torch.empty_like(du), torch.empty_like(du)
+    du, hz = nan_filled((M, N), BF16), nan_filled((M, N), BF16)
     ops.gemm(dy, w2, du, b_mn=True, aux=aux, act=5, out2=hz, drop=e)
     assert torch.equal(hz == 0, (me == 0) | (hz0 == 0)) and rel(hz, hz0.float() * me) < 5e-3
     assert torch.equal(du == 0, (me == 0) | (du0 == 0)) and rel(du, du0.float() * me) < 5e-3
+    check_all(f"dropout act 5 N={N}", {"out": du, "out2": hz},
+              reference(dy, w2, b_mn=True, aux=aux, act=5, out2=True, mult=me))
 
     # the backward's masked operand, from fp32 and from bf16
     x32 = torch.randn(M, N, device="cuda", generator=g)
