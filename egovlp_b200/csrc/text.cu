@@ -276,6 +276,10 @@ extern "C" int egovlp_dropout(const float* x, const float* add, float* y32, void
                               unsigned long long seed, unsigned int site, void* stream) {
   EGOVLP_CHECK_ARG(x && (y32 || y16) && n >= 0 && n % 4 == 0, "dropout: bad args (n must be a multiple of 4)");
   EGOVLP_CHECK_ARG(p >= 0.f && p < 1.f, "dropout: p=%f outside [0, 1)", p);
+  // the kernel moves four elements at a time: float4 for x, add and y32, uint2 for y16
+  EGOVLP_CHECK_ARG(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(add) | reinterpret_cast<uintptr_t>(y32)) &
+                    15) == 0 && (reinterpret_cast<uintptr_t>(y16) & 7) == 0,
+                   "dropout: x, add and y32 must be 16-byte aligned, y16 8-byte aligned");
   if (n == 0) return EGOVLP_OK;
   dropout_kernel<<<(unsigned)((n / 4 + 255) / 256), 256, 0, ST(stream)>>>(x, add, y32, reinterpret_cast<bf16*>(y16), n / 4,
                                                                           p, seed, site);

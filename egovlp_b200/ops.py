@@ -459,6 +459,7 @@ def text_attn_fwd(qkv, mask, out, B, L, H, p_drop=0.0, seed=0, site=0):
 
 
 def text_attn_bwd(qkv, mask, dout, dqkv, B, L, H, q_scale, p_drop=0.0, seed=0, site=0):
+    assert mask.dtype == torch.int64 and mask.is_contiguous()
     call("egovlp_text_attn_bwd", _ptr(qkv), _ptr(mask), _ptr(dout), _ptr(dqkv), B, L, H, C.c_float(q_scale),
          C.c_float(p_drop), C.c_ulonglong(seed), C.c_uint(site), _stream())
 

@@ -254,7 +254,8 @@ int egovlp_video_embed_bwd_det(const float* dx, float* tmp_SD, float* dcls, floa
  *                    >= p_drop * 2^32 (one Philox call per four keys; independent of B, H and L).
  *                    Refused (EGOVLP_ERR_ARG, nothing written): a null pointer, L outside [1, 512], B outside
  *                    [1, 65535], H outside [1, 4096], p_drop outside [0, 1).
- *   dropout        : y = dropout_p(x) (+ add), fp32 [n] -> fp32 y32 and / or bf16 y16 (n % 4 == 0).  The embedding and
+ *   dropout        : y = dropout_p(x) (+ add), fp32 [n] -> fp32 y32 and / or bf16 y16 (n % 4 == 0; x, add, y32 16-byte
+ *                    and y16 8-byte aligned, else EGOVLP_ERR_ARG before any launch).  The embedding and
  *                    FFN-output dropouts of DistilBERT (reference model/model.py:36 puts the text model in train mode);
  *                    calling it on a gradient with the same (p, seed, site) is the backward.
  *   relu_rows      : out bf16 [rows, D] = relu(x[r*row_stride + :D]) (CLS -> ReLU of txt_proj, model/model.py:73-75)

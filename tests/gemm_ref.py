@@ -139,22 +139,30 @@ def bf16_interval(ref, bound):
     return (ref - bound).to(BF16), (ref + bound).to(BF16)
 
 
+def bf16_ratio(got, ref, bound):
+    """Per element of a bf16 `got`: the error it needs as a fraction of `bound` (<= 1 exactly inside [rn(ref - e),
+    rn(ref + e)], > 1 outside, NaN where got is NaN), and the number of bf16 steps it lies outside that interval."""
+    lo, hi = bf16_interval(ref, bound)
+    g, lo_o, hi_o = _ordered_bf16(got), _ordered_bf16(lo), _ordered_bf16(hi)
+    outside = (lo_o - g).clamp_min(0) + (g - hi_o).clamp_min(0)       # bf16 steps outside the interval
+    # the error the result needs: 0 if it is ref rounded, else the distance from ref to the rounding boundary
+    # between got and its neighbour towards ref; as a fraction of the bound, <= 1 exactly inside the interval
+    r_o = _ordered_bf16(ref.to(BF16))
+    nb = _from_ordered(g + torch.sign(r_o - g))
+    need = torch.where(g == r_o, 0.0, ((got.double() + nb.double()) / 2 - ref).abs())
+    ratio = need / bound.clamp_min(1e-300)
+    ratio = torch.where(outside > 0, ratio.clamp_min(1 + 1e-9), ratio.clamp_max(1.0))
+    return ratio.masked_fill(got.isnan(), float("nan")), outside
+
+
 def check(name, got, want):
     """`got` (bf16 or fp32) against want = (fp64 value, bound), element by element, as the module docstring says."""
     ref, bound = want
     assert got.shape == ref.shape, (name, got.shape, ref.shape)
     if got.dtype == BF16:
         lo, hi = bf16_interval(ref, bound)
-        g, lo_o, hi_o = _ordered_bf16(got), _ordered_bf16(lo), _ordered_bf16(hi)
-        outside = (lo_o - g).clamp_min(0) + (g - hi_o).clamp_min(0)       # bf16 steps outside the interval
-        # the error the result needs: 0 if it is ref rounded, else the distance from ref to the rounding boundary
-        # between got and its neighbour towards ref; as a fraction of the bound, <= 1 exactly inside the interval
-        r_o = _ordered_bf16(ref.to(BF16))
-        nb = _from_ordered(g + torch.sign(r_o - g))
-        need = torch.where(g == r_o, 0.0, ((got.double() + nb.double()) / 2 - ref).abs())
-        ratio = need / bound.clamp_min(1e-300)
-        ratio = torch.where(outside > 0, ratio.clamp_min(1 + 1e-9), ratio.clamp_max(1.0))
-        worst, at = _worst(name, ratio.masked_fill(got.isnan(), float("nan")))
+        ratio, outside = bf16_ratio(got, ref, bound)
+        worst, at = _worst(name, ratio)
         assert not bool(outside.any()) and worst <= 1.0, (
             f"{name}: {int((outside > 0).sum())} elements outside their interval; at {at}: got {got[at].item()}, "
             f"interval [{lo[at].item()}, {hi[at].item()}], exact {ref[at].item()}, bound {bound[at].item():.3e}")

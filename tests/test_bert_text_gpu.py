@@ -276,10 +276,9 @@ def test_bert_dropout_vs_oracle_fed_with_the_masks(L):
     """Train-mode dropout at all four sites (embeddings 0, attention probabilities 1 + 2 i, FFN output 2 + 2 i,
     attention output dense 1 + 2 n + i): reproducible under torch.manual_seed, different from p = 0, and equal to the
     oracle fed with the regenerated masks; gradients by cosine > 0.995."""
-    from egovlp_b200 import engine, ops, synthetic as syn
+    from egovlp_b200 import engine, synthetic as syn
     from oracle import bert_port as bp
-    from test_dropout_gpu import _extract_attention_multiplier
-    from test_text_long_gpu import multiplier
+    from philox_ref import flat_multiplier, long_attn_keep, multiplier, short_attn_keep
     dims = tiny_dims()
     sd = {k: v for k, v in syn.seeded_state_dict(dims, seed=4, video=False, proj=True).items()
           if not k.startswith("vid_proj")}
@@ -299,16 +298,14 @@ def test_bert_dropout_vs_oracle_fed_with_the_masks(L):
     assert torch.equal(a, b) and not torch.equal(a, c) and not torch.equal(a, det)
     torch.manual_seed(7)
     seed = int(torch.randint(0, 2 ** 62, (1,)).item())
-    ones = torch.ones(B * L * D, device="cuda")
 
-    def hidden(site):
-        return ops.dropout(ones, p_hid, seed, site, y32=torch.empty_like(ones))[0].view(B, L, D).cpu()
+    def hidden(site):                                  # the host Philox streams (tests/philox_ref.py)
+        return flat_multiplier((B, L, D), p_hid, seed, site).float()
 
     drop = {"emb": hidden(0)}
     for i in range(n):
-        att = (_extract_attention_multiplier(B, L, H, p_att, seed, 1 + 2 * i) if L <= 64
-               else multiplier(seed, 1 + 2 * i, p_att, B, H, L))
-        drop[("att", i)] = att.float().cpu()
+        keep = (short_attn_keep if L <= engine.TEXT_ATTN_SHORT_MAX_L else long_attn_keep)(p_att, seed, 1 + 2 * i, B, H, L)
+        drop[("att", i)] = multiplier(keep, p_att).float()
         drop[("ffn", i)] = hidden(2 + 2 * i)
         drop[("so", i)] = hidden(1 + 2 * n + i)
     p_cpu = {k: v.clone().requires_grad_(True) for k, v in sd.items()}

@@ -1,5 +1,5 @@
-"""Per-kernel reference tests of the video patch-embedding front end (embed.cu), the text tower's small kernels and its
-attention (text.cu).  Whole-tower tests check these kernels only through twelve bf16 blocks, at tolerances sized for
+"""Per-kernel reference tests of the video patch-embedding front end (embed.cu) and the text tower's small kernels
+(text.cu; its attention is checked in test_text_attention_gpu.py).  Whole-tower tests check these kernels only through twelve bf16 blocks, at tolerances sized for
 that, where a bug in one kernel or one branch is diluted or never runs.
 
 Each reference is the same operation written plainly in torch, computed in float64 on the GPU from the same bf16 / fp32
@@ -9,12 +9,9 @@ values the kernel reads.  The bound follows from what the kernel does:
   * reductions stay within |got - ref| <= rel * sum|terms| element-wise (`assert_sum_bound`): the error of an fp32 sum
     scales with the magnitudes it adds, not with its (possibly cancelled) result, and one relative L2 over the whole
     tensor would let a single wrong element through;
-  * attention is checked per (b, h, query row) (`assert_rows_close`), so that one wrong row cannot hide among
-    thousands of correct ones.
-Each check prints its worst element or row as a fraction of its bound (run with -s to see them).
-
-Not tested: attention masks with no valid key at all.  The tokenizer always emits [CLS] and [SEP], and for such a row
-the kernel returns NaN (0 / 0 in the softmax), as the masked_fill(-inf) softmax of the reference does."""
+  * GEMM outputs are also checked per row (`assert_rows_close`), so that one wrong row cannot hide among thousands of
+    correct ones.
+Each check prints its worst element or row as a fraction of its bound (run with -s to see them)."""
 import pytest
 import torch
 from gemm_ref import check, reference
@@ -236,48 +233,3 @@ def test_relu_rows_forward_and_backward_are_exact(ops, cls_only):
     assert torch.equal(got, xg.grad)
     if cls_only:                  # only the CLS token rows (row index a multiple of L) are written
         assert torch.all(dx.view(B, L, D)[:, 1:] == sentinel)
-
-
-# ---------------------------------------------------------------------------------------------------------- C. text attention
-def key_lengths(B, L, seed):
-    """Valid-key counts: sample 0 all keys, sample 1 a single key, sample 2 on a 32-key boundary, the rest random."""
-    lens = torch.randint(1, L + 1, (B,), generator=torch.Generator().manual_seed(seed))
-    lens[0], lens[1], lens[2] = L, 1, (L - 1) // 32 * 32 or L
-    return lens
-
-
-# L = 65..128 runs the third and fourth keys per lane (dp_local[2..3]); L = 128, H = 12 (the model's head count) is the
-# largest shared-memory layout (about 197 KiB in the backward)
-@pytest.mark.parametrize("H", [1, 12])
-@pytest.mark.parametrize("L", [1, 2, 31, 32, 33, 64, 65, 97, 128])
-def test_text_attention_matches_fp64_row_by_row(ops, L, H):
-    B, D, q_scale = 32, 64 * H, 0.125
-    g = torch.Generator(device="cuda").manual_seed(1000 + L * 13 + H)
-    x = torch.randn(B * L, 3 * D, generator=g, device="cuda")
-    x[:, :D] *= 0.25                                  # q pre-scaled: scores of unit-ish spread
-    qkv = x.to(BF16)
-    dout = torch.randn(B * L, D, generator=g, device="cuda").to(BF16)
-    lens = key_lengths(B, L, L * 7 + H).cuda()
-    mask = (torch.arange(L, device="cuda")[None, :] < lens[:, None]).to(torch.int64)
-    out = nan_filled((B * L, D), BF16)
-    ops.text_attn_fwd(qkv, mask, out, B, L, H)
-    dqkv = nan_filled((B * L, 3 * D), BF16)
-    ops.text_attn_bwd(qkv, mask, dout, dqkv, B, L, H, q_scale)
-
-    xr = qkv.double().requires_grad_(True)
-    q, k, v = (xr.view(B, L, 3, H, 64)[:, :, i].permute(0, 2, 1, 3) for i in range(3))
-    key_bias = torch.zeros(B, 1, 1, L, device="cuda", dtype=F64).masked_fill(mask.view(B, 1, 1, L) == 0, float("-inf"))
-    ref = torch.softmax(q @ k.transpose(-1, -2) + key_bias, dim=-1) @ v         # [B, H, L, 64]
-    ref.backward(dout.double().view(B, L, H, 64).permute(0, 2, 1, 3))
-
-    def heads(t, part=None):                          # [B*L, (3,) H*64] -> [B, H, L, 64]
-        t = t.view(B, L, 3, H, 64)[:, :, part] if part is not None else t.view(B, L, H, 64)
-        return t.permute(0, 2, 1, 3)
-
-    tag = f"L={L} H={H}"
-    assert_rows_close(f"text_attn out {tag}", heads(out), ref.detach(), rtol=5e-3)
-    assert_rows_close(f"text_attn dq {tag}", heads(dqkv, 0), q_scale * heads(xr.grad, 0), rtol=1e-2)
-    assert_rows_close(f"text_attn dk {tag}", heads(dqkv, 1), heads(xr.grad, 1), rtol=1e-2)
-    assert_rows_close(f"text_attn dv {tag}", heads(dqkv, 2), heads(xr.grad, 2), rtol=1e-2)
-    padded = dqkv.view(B, L, 3, D)[:, :, 1:][mask == 0]                          # dk, dv of padded keys
-    assert torch.all(padded == 0), f"{tag}: padded keys got nonzero dk / dv"

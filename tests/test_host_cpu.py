@@ -59,6 +59,40 @@ def test_gemm_refuses_misaligned_epilogue_tensors(field, value, msg):
                   C.c_longlong(K), M, N, K, C.byref(e), 1, None)
 
 
+@pytest.mark.parametrize("field,value", [("x", 0x10004), ("add", 0x20008), ("y32", 0x30004), ("y16", 0x40004),
+                                         ("y16", 0x40002)])
+def test_dropout_refuses_misaligned_pointers(field, value):
+    """egovlp_dropout reads x / add and writes y32 as float4, y16 as four bf16 at once: a base off 16 (8) bytes must be
+    refused before any launch.  Made-up addresses, so only where no GPU is visible."""
+    if torch.cuda.is_available():
+        pytest.skip("made-up device addresses: not passed where a GPU is visible")
+    import ctypes as C
+    from egovlp_b200 import _lib
+    ptrs = {"x": 0x10000, "add": 0x20000, "y32": 0x30000, "y16": 0x40000}
+    ptrs[field] = value
+    with pytest.raises(_lib.EgovlpError, match="aligned"):
+        _lib.call("egovlp_dropout", *(C.c_void_p(ptrs[k]) for k in ("x", "add", "y32", "y16")), C.c_longlong(1024),
+                  C.c_float(0.1), C.c_ulonglong(1), C.c_uint(0), None)
+
+
+def test_text_attn_bwd_refuses_a_mask_that_is_not_contiguous_int64(monkeypatch):
+    """The kernel reads the mask as int64 [B, L]: an int32 or strided mask would be read past its end or at the wrong
+    keys, so ops.text_attn_bwd refuses it, as the forward does, before the C call."""
+    from egovlp_b200 import ops
+    reached = []
+    monkeypatch.setattr(ops, "call", lambda name, *args: reached.append(name))
+    monkeypatch.setattr(ops, "_stream", lambda: None)
+    B, L, H = 2, 8, 1
+    qkv, dqkv = torch.zeros(B * L, 3 * 64 * H, dtype=torch.bfloat16), torch.zeros(B * L, 3 * 64 * H, dtype=torch.bfloat16)
+    dout = torch.zeros(B * L, 64 * H, dtype=torch.bfloat16)
+    for bad in (torch.ones(B, L, dtype=torch.int32), torch.ones(L, B, dtype=torch.int64).t()):
+        with pytest.raises(AssertionError):
+            ops.text_attn_bwd(qkv, bad, dout, dqkv, B, L, H, 0.125)
+    assert not reached
+    ops.text_attn_bwd(qkv, torch.ones(B, L, dtype=torch.int64), dout, dqkv, B, L, H, 0.125)
+    assert reached == ["egovlp_text_attn_bwd"]
+
+
 def test_state_dict_contract_matches_reference_keys():
     from egovlp_b200 import synthetic as syn
     from egovlp_b200.model.model import FrozenInTime

@@ -8,13 +8,14 @@ csrc/text_attention.cu) and the tower that dispatches to it for L > 128.
     argument refusals and the position-table check of the tower;
   * the tower against the golden and, at DistilBERT-base geometry, against the fp32 oracle on the GPU; dropout through
     the tower; one FrozenInTime training step with a 300-token caption."""
-import numpy as np
 import pytest
 import torch
 
 from conftest import load_golden
 from divided_attention_ref import Q_SCALE, SENTINEL, SLACK, U, _with_sentinels
-from kernel_checks import BF16, F32, F64, assert_bits_equal, assert_elementwise_bound, nan_filled
+from kernel_checks import BF16, F32, assert_bits_equal, assert_elementwise_bound, nan_filled
+from philox_ref import long_attn_keep, multiplier as philox_multiplier
+from text_attention_ref import make_inputs, plant_maxima, reference
 
 P_ORDER_LAYER = ("attention.q_lin", "attention.k_lin", "attention.v_lin", "attention.out_lin")
 
@@ -76,83 +77,14 @@ def test_oracle_vs_distilbert_long_golden():
             torch.testing.assert_close(h[bi, li], g[f"{tag}_rows"][i], rtol=1e-4, atol=1e-5)
 
 
-# ------------------------------------------------------------------------------------------------ host Philox
-_M32 = np.uint64(0xFFFFFFFF)
-
-
-def philox4x32_10(key, ctr):
-    """common.cuh philox4x32_10 on uint64 numpy arrays of counters -> the four 32-bit words."""
-    k0, k1 = np.uint64(key & 0xFFFFFFFF), np.uint64(key >> 32)
-    c0, c1 = ctr & _M32, ctr >> np.uint64(32)
-    c2, c3 = np.full_like(ctr, 0x2B7E1516), np.full_like(ctr, 0x28AED2A6)
-    for _ in range(10):
-        p0, p1 = np.uint64(0xD2511F53) * c0, np.uint64(0xCD9E8D57) * c2
-        c0, c1, c2, c3 = (p1 >> np.uint64(32)) ^ c1 ^ k0, p1 & _M32, (p0 >> np.uint64(32)) ^ c3 ^ k1, p0 & _M32
-        k0, k1 = (k0 + np.uint64(0x9E3779B9)) & _M32, (k1 + np.uint64(0xBB67AE85)) & _M32
-    return c0, c1, c2, c3
-
-
+# ------------------------------------------------------------------------------------------------ kernel harness
 def keep_mask(seed, site, p, B, H, L):
-    """The documented keep mask of text_attn_long_*: bool [B, H, L(i), L(j)]."""
-    key = (seed ^ ((0x9E3779B97F4A7C15 * (site + 1)) & 0xFFFFFFFFFFFFFFFF)) & 0xFFFFFFFFFFFFFFFF
-    t = float(np.float32(p)) * 4294967296.0
-    thresh = 0xFFFFFFFF if t >= 4294967295.0 else int(t)
-    b, h, i, jg = np.meshgrid(np.arange(B, dtype=np.uint64), np.arange(H, dtype=np.uint64), np.arange(L, dtype=np.uint64),
-                              np.arange((L + 3) // 4, dtype=np.uint64), indexing="ij")
-    words = philox4x32_10(key, ((b * np.uint64(4096) + h) * np.uint64(512) + i) * np.uint64(128) + jg)
-    keep = np.stack([w >= np.uint64(thresh) for w in words], -1).reshape(B, H, L, -1)[..., :L]
-    return torch.from_numpy(keep)
+    """The documented keep mask of text_attn_long_*: bool [B, H, L(i), L(j)] (tests/philox_ref.py)."""
+    return long_attn_keep(p, seed, site, B, H, L)
 
 
 def multiplier(seed, site, p, B, H, L):
-    return keep_mask(seed, site, p, B, H, L).double() / (1 - p)
-
-
-# ------------------------------------------------------------------------------------------------ kernel harness
-def reference(qkv, dout, mask, B, L, H, q_scale, mult=None):
-    """float64 masked attention (dropout multipliers `mult` [B, H, L, L] on the probabilities) and the magnitude sums
-    of the bounds (DESIGN section 6 forms, as tests/divided_attention_ref.py)."""
-    x = qkv.to(F64).view(B, L, 3, H, 64).permute(2, 0, 3, 1, 4)
-    q, k, v = x[0], x[1], x[2]
-    do = dout.to(F64).view(B, L, H, 64).permute(0, 2, 1, 3)
-    valid = mask.bool().view(B, 1, 1, L)
-    s = (q @ k.transpose(-1, -2)).masked_fill(~valid, float("-inf"))
-    lse = torch.logsumexp(s, -1)
-    p = torch.exp(s - lse[..., None])
-    m = mult.to(qkv.device) if mult is not None else torch.ones((), dtype=F64, device=qkv.device)
-    pd = p * m
-    o = pd @ v
-    pv = pd @ v.abs()
-    dp = (do @ v.transpose(-1, -2)) * m
-    delta = (do * o).sum(-1, keepdim=True)
-    ds = p * (dp - delta)
-    e = (do.abs() * (pv + 2 * o.abs())).sum(-1, keepdim=True)
-    w = p * ((dp - delta).abs() + e)
-    lse_t = (q.abs() @ k.abs().transpose(-1, -2)).masked_fill(~valid, 0.0).amax(-1)
-    rows = lambda t: t.permute(0, 2, 1, 3).reshape(B * L, H * 64)
-    return {"out": rows(o), "out_t": rows(pv), "lse": lse, "lse_t": lse_t,
-            "dq": rows(q_scale * (ds @ k)), "dq_t": rows(q_scale * (w @ k.abs())),
-            "dk": rows(ds.transpose(-1, -2) @ q), "dk_t": rows(w.transpose(-1, -2) @ q.abs()),
-            "dv": rows(pd.transpose(-1, -2) @ do), "dv_t": rows(pd.transpose(-1, -2) @ do.abs())}
-
-
-def make_inputs(B, L, H, seed):
-    g = torch.Generator(device="cuda").manual_seed(seed)
-    D = 64 * H
-    x = torch.randn(B * L, 3 * D, generator=g, device="cuda")
-    x[:, :D] *= Q_SCALE
-    return x.to(BF16), torch.randn(B * L, D, generator=g, device="cuda").to(BF16)
-
-
-def plant_last_tile_maxima(qkv, mask, B, L, H, score=18.0):
-    """Every third query row points at its sample's last valid key (in the last valid key tile), `score` above the
-    rest: the running maximum changes in the last tile, so the online rescaling is exercised."""
-    x = qkv.float().view(B, L, 3, H, 64)
-    for b in range(B):
-        last = int(mask[b].nonzero().max())
-        kk = x[b, last, 1]                                         # [H, 64]
-        x[b, ::3, 0] = (kk * (score / kk.pow(2).sum(-1, keepdim=True)))[None]
-    return x.reshape(B * L, 3 * H * 64).to(BF16)
+    return philox_multiplier(keep_mask(seed, site, p, B, H, L), p)
 
 
 def masks_for(L):
@@ -205,7 +137,7 @@ def test_text_attn_long_vs_fp64(ops, L, H):
     mask = masks_for(L)
     B = mask.shape[0]
     qkv, dout = make_inputs(B, L, H, seed=L * 31 + H)
-    qkv = plant_last_tile_maxima(qkv, mask, B, L, H)
+    qkv = plant_maxima(qkv, mask, B, L, H)        # in the last valid key tile
     out, lse, dqkv = run_long(ops, qkv, dout, mask, B, L, H)
     check(f"L={L} H={H}", qkv, dout, mask, out, lse, dqkv, B, L, H)
 
